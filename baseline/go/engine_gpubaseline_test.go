@@ -1,4 +1,4 @@
-// engine_gpubaseline_test.go -- CPU baseline harness for the B200 CheckResources evaluator (cerbos_b200).
+// engine_gpubaseline_test.go -- CPU baseline harness for the H100 CheckResources evaluator (cerbos_b200).
 //
 // Drop this file into internal/engine/ of a cerbos/cerbos checkout (it needs the module's own internal packages and its
 // module cache; `go test` of the package then builds it).  It times the reference's own engine -- engine.Check, the code

@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
-"""bench.py -- CheckResources decisions/sec of the B200 evaluator (BASELINE.json metric).
+"""bench.py -- CheckResources decisions/sec of the H100 evaluator (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload C2] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload C2] [--impl ours|reference] [--dump-outputs DIR]
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...       (N > 1, one rank per GPU)
 
 A *step* is `batches_per_step` passes of the hot path (rule-table scan + CEL condition evaluation), each over one
@@ -18,8 +18,13 @@ A C2 (configs[1]) measurement rides along as `secondary` at N = 1.
   e2e       the same metric through the host-buffer C-ABI call cgpu_check (pinned host columns -> H2D ->
             kernel -> D2H -> effect bytes), i.e. what engine.Check would pay per call
   roofline  algorithmic bytes / launch (SURVEY.md 8(d): C3 197 B, C2 73 B per request) over the mean kernel duration vs the
-            measured HBM copy bandwidth (MEASURED_PEAKS.json)
+            measured HBM copy bandwidth (MEASURED_PEAKS.json; without it the H100 SXM data sheet's 3.35 TB/s)
   cpu_baseline  oracle/c/check_ref.c (a plain-C port of the reference algorithm) on all host cores
+
+--dump-outputs DIR writes, after the timed steps, the decisions of the last step as float32 .npy files (1 = ALLOW,
+2 = DENY; a fixed, seeded sample of requests of every batch that step evaluated) and the sampled request indices, at
+most about 48 MB in all.  Inputs are generated from fixed seeds, so two builds run with the same arguments can be
+compared output for output.
 
 --impl reference times that CPU port alone (the Go toolchain needed for the reference's own engine is not
 in this image; see DESIGN.md).
@@ -53,7 +58,7 @@ def load_peaks():
                 return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3; not a measured figure)"
 
 
 class ClockSampler:
@@ -309,27 +314,6 @@ def run_reference(args):
     }))
 
 
-def ncu_traffic(workload: str, n: int):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one launch of the dominant kernel, scaled to n requests, from the
-    committed `ncu --set full` capture of this workload's kernel (profiles/; None if there is none)."""
-    files = {"C2": ("r1_final_check_kernel_ncu_full.json", 1 << 20), "C3": ("r2_C3_check_kernel_ncu_full.json", 1 << 22),
-             "C5": ("r2_C5_cb_spec_uc_global_ncu_full.json", 1 << 18)}
-    if workload not in files:
-        return None
-    name, n_cap = files[workload]
-    try:
-        with open(os.path.join(ROOT, "profiles", name)) as f:
-            d = json.load(f)
-        if "_traffic_bytes_per_launch" in d:
-            per = float(d["_traffic_bytes_per_launch"])
-        else:
-            mult = {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0}
-            per = sum(float(d[k]["value"]) * mult[d[k]["unit"]] for k in ("dram__bytes_read.sum", "dram__bytes_write.sum"))
-        return per * (n / n_cap)
-    except (OSError, KeyError, ValueError):
-        return None
-
-
 def verify_images(w, blob, host_batches, images, kbytes):
     """Result images against the C port of the reference algorithm (oracle/): bit for bit over every request up to 2^24
     per batch, beyond that over a striped sample (every 16th run of 65 536 requests) as BASELINE.md 2.4 prescribes.
@@ -358,6 +342,20 @@ def verify_images(w, blob, host_batches, images, kbytes):
     return bad, cmp
 
 
+def dump_decisions(out_dir, wname, images, n, K, kbytes, budget=48 << 20):
+    """Writes <workload>_batch<j>_effects.npy (float32 [rows, K]: 1 ALLOW, 2 DENY) for every batch j in `images` and
+    <workload>_rows.npy (float64: the request indices of those rows): a seeded sample of rows, the same on every run with
+    the same request count, actions and batch set, at most `budget` bytes in all."""
+    os.makedirs(out_dir, exist_ok=True)
+    n_rows = max(1, min(n, budget // (4 * K * len(images) + 8)))
+    rows = np.sort(np.random.default_rng(0x5EED).choice(n, size=n_rows, replace=False))
+    np.save(os.path.join(out_dir, f"{wname}_rows.npy"), rows.astype(np.float64))
+    for j, img in sorted(images.items()):
+        bm = np.asarray(img).reshape(n, kbytes)[rows]
+        bits = np.unpackbits(bm, axis=1, bitorder="little")[:, :K]
+        np.save(os.path.join(out_dir, f"{wname}_batch{j}_effects.npy"), np.where(bits == 1, 1, 2).astype(np.float32))
+
+
 def measure(args, ctx, w, blob, enc, table, dev, rank, world, local_rank, n, primary=True):
     """Times the device-resident path of one workload; returns the result fragment (see main)."""
     import torch
@@ -373,6 +371,7 @@ def measure(args, ctx, w, blob, enc, table, dev, rank, world, local_rank, n, pri
         host_batches.append(hb)
         batches.append(DeviceBatch(hb, dev))
     footprint = sum(b.nbytes() for b in batches)
+    l2_mb = getattr(torch.cuda.get_device_properties(dev), "L2_cache_size", 0) / 1e6
     kbytes = batches[0].kbytes
     calls = [b.prepare(table, NOW_NS) for b in batches]
     views = [b.bitmap[: n * kbytes] for b in batches]
@@ -428,6 +427,11 @@ def measure(args, ctx, w, blob, enc, table, dev, rank, world, local_rank, n, pri
     gathered = [torch.empty(world * n * kbytes, dtype=torch.uint8, device=dev) for _ in range(n_buf)] if (world > 1 and primary and pg is None) else None
     pending = []
     it = [0]          # launches issued so far (warm-up included): numbers the gather steps
+
+    def image(j):   # this rank's packed result bitmap of batch j (1 bit per decision, bit set = ALLOW)
+        if pg is not None:
+            return pg.read(j)[rank * n * kbytes:(rank + 1) * n * kbytes]
+        return batches[j].bitmap[: n * kbytes].cpu().numpy()
 
     def launch():
         g = it[0]
@@ -521,6 +525,9 @@ def measure(args, ctx, w, blob, enc, table, dev, rank, world, local_rank, n, pri
     launches = ctx.launch_count() - launches0
     for h in stream_hs:
         ctx.sync(h)
+    if args.dump_outputs and primary and rank == 0:
+        # the batches the last timed step evaluated (its m launches, numbered it[0] - m .. it[0] - 1, rotate over n_buf)
+        dump_decisions(args.dump_outputs, w.name, {j: image(j) for j in {g % n_buf for g in range(it[0] - m, it[0])}}, n, K, kbytes)
     if world > 1 and primary:
         tmax = torch.tensor([total_ms], dtype=torch.float64, device=dev)
         dist.all_reduce(tmax, op=dist.ReduceOp.MAX)
@@ -557,12 +564,7 @@ def measure(args, ctx, w, blob, enc, table, dev, rank, world, local_rank, n, pri
         for h in stream_hs:
             ctx.sync(h)
         torch.cuda.synchronize()
-        images = []
-        for j in range(n_buf):
-            if pg is not None:
-                images.append(pg.read(j)[rank * n * kbytes:(rank + 1) * n * kbytes])
-            else:
-                images.append(batches[j].bitmap[: n * kbytes].cpu().numpy())
+        images = [image(j) for j in range(n_buf)]
         bad, compared = verify_images(w, blob, host_batches, images, kbytes)
         if world > 1 and primary:
             tb = torch.tensor([bad], dtype=torch.int64, device=dev)
@@ -581,10 +583,10 @@ def measure(args, ctx, w, blob, enc, table, dev, rank, world, local_rank, n, pri
     res = {
         "value": value, "ms_per_step": per_step_ms, "batches_per_step": m, "requests_per_batch": n, "actions_per_request": K,
         "ms_per_batch": per_step_ms / m, "host_issue_ms_per_batch": host_issue_ms, "streams": n_streams, "gather_mode": gather_mode,
-        "l2": f"rotating {n_buf} distinct batches, {footprint / 1e6:.0f} MB of columns > 126 MB L2", "kernel": kcfg,
+        "l2": f"rotating {n_buf} distinct batches, {footprint / 1e6:.0f} MB of columns; L2 {l2_mb:.0f} MB", "kernel": kcfg,
         "gpu_launches": int(launches),
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": ncu_traffic(w.name, n), "peak_source": peak_src, "algorithmic_bytes_per_launch": algo_bytes,
+                     "peak_source": peak_src, "algorithmic_bytes_per_launch": algo_bytes,
                      "kernel": ("check_kernel<false,2> (general body draining the deferral list; timed as the whole call)" if not kernel_dominates else
                                 ("cb_spec_uc" if kcfg.get("smem_bytes") else "cb_spec_uc_global") if kcfg.get("unique_conditions") and kcfg.get("table_specialised") else
                                 "cb_spec_tiles" if kcfg.get("table_specialised") else "check_kernel"),
@@ -760,6 +762,8 @@ def main():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-secondary", action="store_true", help="skip the C2 ride-along measurement at N = 1")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write a seeded sample of the last step's decisions as .npy files to DIR")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3
@@ -770,6 +774,16 @@ def main():
     import torch.distributed as dist
     from cerbos_b200 import capi
     import workloads as W
+
+    # kernels the library compiles with NVRTC at table load are cached on disk: keep that cache out of the source tree
+    # and out of the user's home unless the caller chose a directory
+    if "CERBOS_B200_CACHE_DIR" not in os.environ:
+        import atexit
+        import shutil
+        import tempfile
+        cache = tempfile.mkdtemp(prefix="cerbos_b200_nvrtc_")
+        atexit.register(shutil.rmtree, cache, True)
+        os.environ["CERBOS_B200_CACHE_DIR"] = cache
 
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))

@@ -1,8 +1,8 @@
-"""cerbos_b200 -- B200-native batched CheckResources evaluator (the hot path of cerbos/cerbos:
+"""cerbos_b200 -- H100-native batched CheckResources evaluator (the hot path of cerbos/cerbos:
 engine.Check -> ruletable.check -> CEL conditions), behind a C ABI (include/cerbos_b200.h).
 
 Layout
-  csrc/      CUDA kernels (sm_100a) + C ABI            -> _lib/libcerbos_b200.so
+  csrc/      CUDA kernels (sm_90a) + C ABI             -> _lib/libcerbos_b200.so
   capi.py    ctypes binding of the C ABI
   engine.py  Engine.Check mirror (host buffers in, effects out)
   device.py  device-resident batches (torch tensors) for benchmarks / multi-GPU sharding

@@ -1,4 +1,4 @@
-// cb_core.h -- per-request evaluation core of the B200 CheckResources kernels.
+// cb_core.h -- per-request evaluation core of the H100 CheckResources kernels.
 //
 // One thread evaluates one request (principal, resource, K actions) against the flattened rule table:
 //   * scope chains + existence checks      (reference: ruletable.go:611-645, 804-863; index.go:1089-1172)

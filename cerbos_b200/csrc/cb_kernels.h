@@ -1,10 +1,10 @@
-// cb_kernels.h -- device bodies of the CheckResources kernels (sm_100a).
+// cb_kernels.h -- device bodies of the CheckResources kernels (sm_90a).
 //
 // Included twice: by cerbos_b200.cu (ahead-of-time build: every body, generic block walker) and, as embedded text,
 // by the translation unit the library compiles with NVRTC when a table is loaded (CB_LEAN_ONLY: lean bodies only,
 // with the straight-line block evaluators cb_specialize.h generates from that table).
 //
-// Kernel design (B200):
+// Kernel design (H100):
 //   * persistent grid: (SM count x resident CTAs) CTAs of 256 threads loop over 256-request tiles;
 //   * the flattened rule table image (row blocks, scope tables, bytecode, constants; KBs) is staged ONCE per CTA
 //     into shared memory by the TMA unit: 1-D `cp.async.bulk.shared::cluster.global` copies completing on an

@@ -2,7 +2,7 @@
 
 Restates internal/util/globs_common.go:11-87 (``glob.Compile(expr, ':')`` with the
 lone ``*`` -> ``**`` fix-up at :74-81) over the published syntax of
-github.com/gobwas/glob v0.2.3 (go.mod:42; source not under /root/reference):
+github.com/gobwas/glob v0.2.3 (go.mod:42; source outside the reference tree):
 ``*`` = any run of non-separator chars, ``**`` = any run, ``?`` = one non-separator
 char, ``[abc]``/``[a-z]``/``[!abc]`` classes, ``{a,b}`` alternatives, ``\\`` escape.
 

@@ -1,7 +1,7 @@
 """Encrypted rule-table bundles (`*.crrts`): the stream cipher layer in front of the serialized runtimev1.RuleTable.
 
 The reference decrypts with ``crypto.DecryptChaCha20Poly1305Stream(key, in, out)`` (internal/storage/hub/
-ruletable_bundle.go:56-70) from github.com/cerbos/cloud-api -- a third-party module that is not under /root/reference.  The
+ruletable_bundle.go:56-70) from github.com/cerbos/cloud-api -- a third-party module outside the reference tree.  The
 format restated here was identified on the reference's own fixture (internal/test/testdata/bundle/v2_ruletable/
 bundle.crrts + encryption_key.txt, 48 bytes longer than its 131 518-byte plaintext) and is pinned by it: the STREAM
 construction over ChaCha20-Poly1305 (RFC 8439) --

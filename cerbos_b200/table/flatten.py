@@ -1,6 +1,6 @@
 """RuleTable -> flattened, HBM-resident table blob (host side, once per policy change).
 
-B200-first replacement for the reference's in-memory index
+H100-first replacement for the reference's in-memory index
 (``index.Impl.IndexRules`` internal/ruletable/index/index.go:353-437, the five
 inverted indexes of mem.go:57-220, ``indexRules`` internal/ruletable/ruletable.go:563-601,
 ``compileParentRoleAncestors`` index.go:842-881): instead of hash-map row sets that

@@ -1,5 +1,5 @@
 /*
- * cerbos_b200.h -- C ABI of the B200-native batched CheckResources evaluator.
+ * cerbos_b200.h -- C ABI of the H100-native batched CheckResources evaluator.
  *
  * This is the drop-in boundary for the reference's hot path.  What it replaces (cerbos/cerbos):
  *

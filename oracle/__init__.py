@@ -10,7 +10,7 @@ legs may import or execute anything under ``oracle/``.  Nothing under
 Layers
   oracle/celeval.py   tree-walking CEL evaluator with cel-go v0.27.0 semantics
                       (third-party dependency of the reference, go.mod:45 --
-                      its source is NOT under /root/reference; semantics are
+                      its source is NOT in the reference tree; semantics are
                       restated from the CEL spec and pinned by the reference's
                       own goldens: internal/test/testdata/cel_eval/*.yaml,
                       internal/conditions/cerbos_lib_test.go:26-134).

@@ -1,7 +1,7 @@
 """Tree-walking CEL evaluator with cel-go semantics -- TEST INFRASTRUCTURE (oracle).
 
 Restates the behaviour of ``github.com/google/cel-go v0.27.0`` (go.mod:45 of the
-reference; NOT vendored under /root/reference) as configured by
+reference; NOT vendored in the reference tree) as configured by
 ``conditions.StdEnv`` (internal/conditions/cel.go:62-75): standard CEL,
 heterogeneous equality, CrossTypeNumericComparisons, ext.Strings / Lists /
 Bindings / Encoders / Math / TwoVarComprehensions, plus the Cerbos library
@@ -101,7 +101,7 @@ class Hierarchy:
 
 
 # ---- SPIFFE types (internal/conditions/types/spiffe.go over github.com/spiffe/go-spiffe/v2 v2.x, go.mod -- a third-party
-# dependency that is not under /root/reference: its spiffeid.FromString / TrustDomainFromString / ValidatePath rules are
+# dependency outside the reference tree: its spiffeid.FromString / TrustDomainFromString / ValidatePath rules are
 # restated here from the library's published source and pinned by the reference's TestCerbosLib rows and cel_eval goldens)
 _TD_CHARS = set("abcdefghijklmnopqrstuvwxyz0123456789-._")
 _SEG_CHARS = _TD_CHARS | set("ABCDEFGHIJKLMNOPQRSTUVWXYZ")

@@ -1,6 +1,6 @@
 """Extracts the example rows of the reference's CEL documentation (docs/modules/policies/pages/conditions.adoc) as test
 vectors: every function table there gives, per row, an expression written to hold (evaluate to true) over the section's
-"Test data" request fragment.  Run in the authoring container (needs /root/reference); the output
+"Test data" request fragment.  Needs a cerbos/cerbos source tree (CERBOS_SRC); the output
 tests/golden/conditions_adoc.json is committed, this script is how it was made.
 
     python tests/golden/make_adoc_vectors.py
@@ -9,7 +9,7 @@ import json
 import os
 import re
 
-SRC = "/root/reference/docs/modules/policies/pages/conditions.adoc"
+SRC = os.path.join(os.environ.get("CERBOS_SRC", "."), "docs/modules/policies/pages/conditions.adoc")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "conditions_adoc.json")
 
 

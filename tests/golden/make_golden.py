@@ -2,7 +2,7 @@
 """Extracts the reference's golden TEST VECTORS for the CheckResources hot path
 into compact JSON fixtures under tests/golden/.
 
-Run in the authoring container (needs /root/reference):
+Needs a cerbos/cerbos source tree (CERBOS_SRC, the directory holding internal/):
     python tests/golden/make_golden.py
 
 Sources (all test data, no reference source code is copied):
@@ -30,7 +30,7 @@ import sys
 
 import yaml
 
-REF = "/root/reference/internal"
+REF = os.path.join(os.environ.get("CERBOS_SRC", "."), "internal")
 TD = f"{REF}/test/testdata"
 OUT = os.path.dirname(os.path.abspath(__file__))
 
@@ -255,7 +255,7 @@ def ruletable_bundle():
 
 if __name__ == "__main__":
     if not os.path.isdir(REF):
-        sys.exit("needs /root/reference (authoring container only)")
+        sys.exit("set CERBOS_SRC to a cerbos/cerbos source tree")
     cel_eval()
     cerbos_lib_table()
     engine_cases()

@@ -1,6 +1,6 @@
 // tests/hostsim/hostsim.cpp -- DEBUG AID (test infrastructure, never shipped, never timed).
 // Compiles the kernels' per-request core (cerbos_b200/csrc/cb_core.h) for the host so its logic can be
-// checked against the oracles in this GPU-less container before a gpurun call is spent.  The product
+// checked against the oracles on a machine without a GPU.  The product
 // library (libcerbos_b200.so) contains no such path: without a CUDA device cgpu_init fails.
 #include <cstdint>
 #include <cstring>

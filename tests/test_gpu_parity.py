@@ -597,7 +597,7 @@ def test_decision_metadata_on_gpu():
 
 def test_multi_device_context_shards_a_batch():
     """cgpu_init with several devices in ONE process (SURVEY 8(b)): the table lives on every device, cgpu_check cuts the batch
-    into one index range per device; results index-aligned and equal to the oracle.  Needs >= 2 GPUs (gpurun --gpus 2)."""
+    into one index range per device; results index-aligned and equal to the oracle.  Needs >= 2 GPUs."""
     import torch
     from cerbos_b200 import capi
     import workloads as W

@@ -39,7 +39,7 @@ def test_product_does_not_import_oracle():
 
 def test_runtime_specialisation_compiles_without_a_device():
     """The table-specialised translation unit the library hands to NVRTC at table load (embedded cb_core.h / cb_kernels.h +
-    generated block evaluators, or -- tables with many block shapes -- the unique-condition evaluator) compiles for sm_100a
+    generated block evaluators, or -- tables with many block shapes -- the unique-condition evaluator) compiles for sm_90a
     here, without a GPU -- C5 too (73 distinct conditions, 50 of them leaf programs translated from their bytecode); tables
     that do not qualify say why (a condition building a list in the arena: no translation)."""
     from cerbos_b200 import capi

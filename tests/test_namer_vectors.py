@@ -19,7 +19,8 @@ FQN_SPECIAL = [   # (policy name, fqn function, want) -- namer_test.go:230-278
 ]
 
 
-@pytest.mark.parametrize("name,fn,want", FQN_SPECIAL, ids=[c[0] for c in FQN_SPECIAL])
+# ids: "::" separates the parts of a pytest node id, so it is kept out of parameter ids (the IAM ARN's empty region)
+@pytest.mark.parametrize("name,fn,want", FQN_SPECIAL, ids=[c[0].replace("::", ":_:") for c in FQN_SPECIAL])
 def test_fqn_special_chars(name, fn, want):
     assert fn(name, "default", "a.b.c") == want
 

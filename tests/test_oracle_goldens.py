@@ -1,6 +1,6 @@
 """Pins the CPU oracle against the reference's own golden vectors (SURVEY.md §8c).
 
-Fixtures under tests/golden/ are extracted from /root/reference test data by
+Fixtures under tests/golden/ are extracted from the cerbos/cerbos test data by
 tests/golden/make_golden.py.
 """
 import pytest

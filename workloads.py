@@ -163,7 +163,7 @@ class C1:
 # =========================================================================================== C2
 class C2:
     """10 resource policies x 8 actions, 2 derived roles with CEL on request.resource.attr; batch 2^20.
-    This is the configuration BASELINE.json's metric is quoted on for 1xB200."""
+    This is the configuration BASELINE.json's metric is quoted on for one H100."""
     name = "C2"
     cfg = 2
     actions = [f"a{i}" for i in range(8)]

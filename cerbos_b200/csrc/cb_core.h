@@ -44,8 +44,8 @@ struct TableLayout {
     uint32_t nV, nRP, nS, nP, nR, nAP, nT, n_slots, n_rows;
     uint32_t has_role_policies, has_parent_roles, has_principal_policies;
     uint32_t image_bytes;
-    // "unique condition" image (cb_uc.h): offsets of the two derived sections, number of distinct conditions (0 = none)
-    uint32_t uc_conds_off, uc_rows_off, n_uconds;
+    // "unique condition" image (cb_uc.h): offsets of the three derived sections, number of distinct conditions (0 = none)
+    uint32_t uc_conds_off, uc_rows_off, uc_chain_off, n_uconds;
     uint32_t theap_words;   // 8-byte words in THEAP
     uint32_t uses_runtime;  // a condition reads runtime.effectiveDerivedRoles
 };
@@ -86,6 +86,7 @@ struct TableView {
     CB_HD const uint32_t *dr_name_str() const { return sec<uint32_t>(CB_SEC_DR_NAME_STR); }
     CB_HD const cb_cond *uconds() const { return reinterpret_cast<const cb_cond *>(base + L->uc_conds_off); }     // [n_uconds + 1], entry 0 unused
     CB_HD const U4 *urows() const { return reinterpret_cast<const U4 *>(base + L->uc_rows_off); }                 // [n_rows] 16-byte rows, DENY first per block
+    CB_HD const U4 *uc_chain() const { return reinterpret_cast<const U4 *>(base + L->uc_chain_off); }             // like RES_BLOCK_MAP: one scope-walk step each
 };
 
 enum { CB_MAX_GATHER = 8 };
@@ -2496,142 +2497,145 @@ CB_HD int term_tri(const TableView t, const BatchView &b, const Cols &cols, uint
 // Several conditions of a table usually read the same list attribute (principal groups, allowed groups ...).  The
 // specialised build loads such a list ONCE per request into registers -- length + up to CB_LC elements, normalised so
 // that scalar equality is plain 64-bit equality (-0.0 -> +0.0; padding = a sentinel that equals nothing) -- and every
-// membership / set predicate over it is a fully unrolled, branch-free run of compares.  Lists the cache cannot hold
-// exactly (longer, container / int / NaN elements) raise `slow`: the request goes to the general body.
+// membership / set predicate over it is a fully unrolled run of compares.  Lists the cache cannot hold exactly (longer,
+// container / int / NaN elements) raise `slow`: the request goes to the general body.
+// The element loops stop at `bound`: the longest list among the lanes of the warp (the device build; the host build
+// uses the list's own length), clamped to CB_LC.  It is warp-uniform, so every `if (j < bound)` below is a uniform
+// branch over a constant index (the arrays stay in registers), and positions at or above every lane's length hold only
+// padding: skipping them changes no result.
 enum { CB_LC = 8 };
+CB_HD uint32_t list_bound(uint32_t own) {
+#if defined(__CUDA_ARCH__)
+    return __reduce_max_sync(__activemask(), own);
+#else
+    return own;
+#endif
+}
 #ifndef CB_LIST_KEYS64
 // Lists of interned strings (what set / membership conditions over attributes hold in practice) are cached as their
 // 32-bit string ids: half the registers and compares of the boxed words.  Any other element (number, bool, null,
 // container) makes the list one "this cache cannot hold": the general body decides.
 struct ListRegs {
     uint32_t st, len;        // st 0: cached list; 1: slot ABSENT / ERROR; 2: a list this cache cannot hold exactly; 3: another type
+    uint32_t bound;          // element positions the loops visit (see above)
     uint32_t e[CB_LC];
 };
 static constexpr uint32_t kListPad = 0xFFFFFFFEu;      // never a string id
 static constexpr uint32_t kListNoKey = 0xFFFFFFFFu;    // a scalar that is not a string: equal to no element of a cached list
 static constexpr uint32_t kStringTop = CB_V64_BOX_BASE | CB_V64_STRING;
-CB_HD ListRegs list_load(const TableView t, const BatchView &b, uint64_t x) {
-    ListRegs L;
-    L.st = v64_bad(x) ? 1u : v64_tag(x) == CB_V64_LIST ? 0u : 3u;
-    L.len = 0;
-#if defined(__CUDA_ARCH__)
-#pragma unroll
-#endif
-    for (int j = 0; j < CB_LC; j++) L.e[j] = kListPad;
-    if (L.st == 0) {
-        // length and the first CB_LC element words are requested together (bounded by the end of the heap, not by the
-        // length: one memory round trip instead of two); words beyond the length are discarded below
-        const uint64_t pay = x & 0xFFFFFFFFFFFFull;
-        const bool in_batch = (pay & CB_V64_HEAP_BATCH_BIT) != 0;
-        const uint64_t off = in_batch ? pay & (CB_V64_HEAP_BATCH_BIT - 1) : pay;
-        const uint64_t *p = (in_batch ? b.heap : t.theap()) + off;
-        const uint64_t room = (in_batch ? b.heap_words : (uint64_t)t.L->theap_words) - off;   // words from p to the end of its heap
-        uint64_t w[CB_LC];
-        L.len = (uint32_t)ldg(p);
-#if defined(__CUDA_ARCH__)
-#pragma unroll
-#endif
-        for (int j = 0; j < CB_LC; j++) w[j] = (uint64_t)(j + 1) < room ? ldg(p + 1 + j) : 0ull;
-        bool odd = L.len > CB_LC;
-#if defined(__CUDA_ARCH__)
-#pragma unroll
-#endif
-        for (int j = 0; j < CB_LC; j++) {
-            const bool in = (uint32_t)j < L.len;
-            odd |= in && (uint32_t)(w[j] >> 48) != kStringTop;
-            L.e[j] = in ? (uint32_t)w[j] : kListPad;
-        }
-        L.st = odd ? 2u : 0u;
-    }
-    return L;
-}
-// x in L: the outcome of in_tri() / the IN branch of term_tri() for every input this form decides, `slow` otherwise
-CB_HD int list_in_tri(uint64_t x, const ListRegs &L, bool &slow) {
-    if (v64_bad(x) || L.st == 1) return TRI_E;
-    if (L.st != 0 || v64_tag(x) > CB_V64_STRING || x == CB_V64_CANON_NAN) { slow = true; return TRI_E; }
-    const uint32_t nx = (uint32_t)(x >> 48) == kStringTop ? (uint32_t)x : kListNoKey;   // number / bool / null: in no list of strings
-    bool found = false;
-#if defined(__CUDA_ARCH__)
-#pragma unroll
-#endif
-    for (int j = 0; j < CB_LC; j++) found |= nx == L.e[j];
-    return found ? TRI_T : TRI_F;
-}
+CB_HD uint32_t list_key(uint64_t w) { return (uint32_t)w; }
+CB_HD bool list_elem_odd(uint64_t w) { return (uint32_t)(w >> 48) != kStringTop; }
+static constexpr uint64_t kListBeyondHeap = 0ull;      // a word past the end of the heap: not a string, so the list defers
 #else
 struct ListRegs {
     uint32_t st, len;        // st 0: cached list; 1: slot ABSENT / ERROR; 2: a list this cache cannot hold exactly; 3: another type
+    uint32_t bound;          // element positions the loops visit (see above)
     uint64_t e[CB_LC];
 };
 static constexpr uint64_t kListPad = 0xFFFE000000000001ull;    // box tag 14: never produced by an encoder
 CB_HD uint64_t norm_scalar(uint64_t v) { return v == 0x8000000000000000ull ? 0ull : v; }
+CB_HD uint64_t list_key(uint64_t w) { return norm_scalar(w); }
+CB_HD bool list_elem_odd(uint64_t w) { return v64_tag(w) > CB_V64_STRING || w == CB_V64_CANON_NAN; }
+static constexpr uint64_t kListBeyondHeap = kListPad;          // tag 14: the list defers
+#endif
 CB_HD ListRegs list_load(const TableView t, const BatchView &b, uint64_t x) {
     ListRegs L;
     L.st = v64_bad(x) ? 1u : v64_tag(x) == CB_V64_LIST ? 0u : 3u;
     L.len = 0;
-#if defined(__CUDA_ARCH__)
-#pragma unroll
+#ifdef CB_UC_STUB_LISTS   // tools/uc_variants.sh: no heap loads, no compares (wrong results)
+    L.len = (uint32_t)x & 7u;
+    L.bound = CB_LC;
+    for (int j = 0; j < CB_LC; j++) L.e[j] = (uint32_t)x + j;
+    return L;
 #endif
-    for (int j = 0; j < CB_LC; j++) L.e[j] = kListPad;
+    const uint64_t *p = nullptr;
+    uint64_t room = 0;   // words from p to the end of its heap
     if (L.st == 0) {
         const uint64_t pay = x & 0xFFFFFFFFFFFFull;
         const bool in_batch = (pay & CB_V64_HEAP_BATCH_BIT) != 0;
         const uint64_t off = in_batch ? pay & (CB_V64_HEAP_BATCH_BIT - 1) : pay;
-        const uint64_t *p = (in_batch ? b.heap : t.theap()) + off;
-        const uint64_t room = (in_batch ? b.heap_words : (uint64_t)t.L->theap_words) - off;   // words from p to the end of its heap
-        uint64_t w[CB_LC];
+        p = (in_batch ? b.heap : t.theap()) + off;
+        room = (in_batch ? b.heap_words : (uint64_t)t.L->theap_words) - off;
         L.len = (uint32_t)ldg(p);
-#if defined(__CUDA_ARCH__)
-#pragma unroll
-#endif
-        for (int j = 0; j < CB_LC; j++) w[j] = (uint64_t)(j + 1) < room ? ldg(p + 1 + j) : kListPad;
-        bool odd = L.len > CB_LC;
-#if defined(__CUDA_ARCH__)
-#pragma unroll
-#endif
-        for (int j = 0; j < CB_LC; j++) {
-            const bool in = (uint32_t)j < L.len;
-            odd |= in && (v64_tag(w[j]) > CB_V64_STRING || w[j] == CB_V64_CANON_NAN);
-            L.e[j] = in ? norm_scalar(w[j]) : kListPad;
-        }
-        L.st = odd ? 2u : 0u;
     }
+    // every element word below the bound is requested at once (bounded by the end of the heap, not by this lane's
+    // length); words beyond the length are discarded below
+    L.bound = list_bound(L.len < CB_LC ? L.len : CB_LC);
+    uint64_t w[CB_LC];
+#if defined(__CUDA_ARCH__)
+#pragma unroll
+#endif
+    for (int j = 0; j < CB_LC; j++) {
+        w[j] = kListBeyondHeap;
+        if ((uint32_t)j < L.bound && (uint64_t)(j + 1) < room) w[j] = ldg(p + 1 + j);
+    }
+    bool odd = L.len > CB_LC;
+#if defined(__CUDA_ARCH__)
+#pragma unroll
+#endif
+    for (int j = 0; j < CB_LC; j++) {
+        const bool in = (uint32_t)j < L.len;
+        odd |= in && list_elem_odd(w[j]);
+        L.e[j] = in ? list_key(w[j]) : kListPad;
+    }
+    if (L.st == 0) L.st = odd ? 2u : 0u;
     return L;
 }
+// x in L: the outcome of in_tri() / the IN branch of term_tri() for every input this form decides, `slow` otherwise
 CB_HD int list_in_tri(uint64_t x, const ListRegs &L, bool &slow) {
+#ifdef CB_UC_STUB_LISTS
+    return (uint32_t)x == L.e[0] ? TRI_T : TRI_F;
+#endif
     if (v64_bad(x) || L.st == 1) return TRI_E;
     if (L.st != 0 || v64_tag(x) > CB_V64_STRING || x == CB_V64_CANON_NAN) { slow = true; return TRI_E; }
+#ifndef CB_LIST_KEYS64
+    const uint32_t nx = (uint32_t)(x >> 48) == kStringTop ? (uint32_t)x : kListNoKey;   // number / bool / null: in no list of strings
+#else
     const uint64_t nx = norm_scalar(x);
+#endif
     bool found = false;
 #if defined(__CUDA_ARCH__)
 #pragma unroll
 #endif
-    for (int j = 0; j < CB_LC; j++) found |= nx == L.e[j];
+    for (int j = 0; j < CB_LC; j++)
+        if ((uint32_t)j < L.bound) found |= nx == L.e[j];
     return found ? TRI_T : TRI_F;
 }
-#endif
-// hasIntersection(A, B) / isSubset(A, B): the INTERSECTS / SUBSET branch of term_tri()
-CB_HD int list_set_tri(bool subset, const ListRegs &A, const ListRegs &B, bool &slow) {
-    if (A.st == 1 || B.st == 1) return TRI_E;
-    if (A.st == 3 || B.st == 3) return TRI_E;
-    if (A.st == 2 || B.st == 2) { slow = true; return TRI_E; }
-    bool any_hit = false, all_hit = true;
+// Which elements of A occur in B: bit i for element i (i < A.len).  Every set predicate over the same two list slots
+// reads this one mask (cb_specialize.h: generate_uc): one compare grid per pair instead of one per predicate.
+CB_HD uint32_t list_mask(const ListRegs &A, const ListRegs &B) {
+    uint32_t m = 0;
 #if defined(__CUDA_ARCH__)
 #pragma unroll
 #endif
     for (int i = 0; i < CB_LC; i++) {
+        if ((uint32_t)i >= A.bound) continue;
         bool hit = false;
 #if defined(__CUDA_ARCH__)
 #pragma unroll
 #endif
-        for (int j = 0; j < CB_LC; j++) hit |= A.e[i] == B.e[j];
-        const bool valid = (uint32_t)i < A.len;   // padding of A would "hit" the padding of B
-        any_hit |= valid && hit;
-        all_hit &= !valid || hit;
+        for (int j = 0; j < CB_LC; j++)
+            if ((uint32_t)j < B.bound) hit |= A.e[i] == B.e[j];
+        m |= (uint32_t)(hit && (uint32_t)i < A.len) << i;   // padding of A would "hit" the padding of B
     }
-    return (subset ? all_hit : any_hit) ? TRI_T : TRI_F;
+    return m;
+}
+// the INTERSECTS / SUBSET branch of term_tri() from m = list_mask(A, B): isSubset(A, B) is "every element of A hit",
+// hasIntersection(A, B) -- and hasIntersection(B, A), the status tests being symmetric -- is "some element hit"
+CB_HD int list_set_tri(bool subset, const ListRegs &A, const ListRegs &B, uint32_t m, bool &slow) {
+#ifdef CB_UC_STUB_LISTS
+    return (A.e[0] == B.e[subset] + m) ? TRI_T : TRI_F;
+#endif
+    if (A.st == 1 || B.st == 1) return TRI_E;
+    if (A.st == 3 || B.st == 3) return TRI_E;
+    if (A.st == 2 || B.st == 2) { slow = true; return TRI_E; }
+    return (subset ? m == (1u << A.len) - 1u : m != 0u) ? TRI_T : TRI_F;   // st 0: len <= CB_LC
 }
 // attribute.startsWith / endsWith / contains(constant string) through the per-string predicate word (BatchView::strpred)
 CB_HD int strpred_tri(const BatchView &b, uint64_t x, uint32_t p) {
+#ifdef CB_UC_STUB_STRPRED   // tools/uc_variants.sh: attribution of kernel time (wrong results)
+    return (int)((x >> p) & 1u);
+#endif
     if (v64_bad(x)) return TRI_E;
     if (v64_tag(x) != CB_V64_STRING) return TRI_E;
     return (int)((ldg(b.strpred + (uint32_t)(x & 0xFFFFFFFFu)) >> p) & 1u);
@@ -3447,31 +3451,32 @@ CB_HD uint32_t uc_row_pairs(const U4 r, const RP rp, const CondWord v, const uin
     const uint32_t rc = miss ? 0u : (uint32_t)(rp >> r.w) & role_all;
     return r.x * rc;
 }
-// The scope-chain walk of the unique-condition body: per block the DENY rows, then the ALLOW rows, each row three or
-// four ALU operations on registers.  RP: the role table word (32 bits when every role field fits, else 64);
-// kForm: how the rows name their conditions (known when the kernel is generated for a table).
+// The scope-chain walk of the unique-condition body: per scope the DENY rows, then the ALLOW rows, each row three or
+// four ALU operations on registers.  One 16-byte step record per scope (cb_uc.h: the chain descriptors, indexed like
+// RES_BLOCK_MAP) gives the row ranges and the next scope of the chain, so a scope costs one table load ahead of its rows.
+// RP: the role table word (32 bits when every role field fits, else 64); kForm: how the rows name their conditions
+// (known when the kernel is generated for a table).
 template <typename RP, int kForm, typename Rows>
-CB_HD uint32_t uc_walk(const TableView t, const BatchView &b, const Rows rows, const RP rp, const CondWord val, const uint32_t r0, const uint32_t bm_base,
+CB_HD uint32_t uc_walk(const TableView t, const Rows rows, const RP rp, const CondWord val, const uint32_t r0, const uint32_t bm_base,
                        const uint32_t aset_base, const uint32_t role_all, uint32_t alive) {
-    (void)b;
     uint32_t allow_pairs = 0;
-    for (uint32_t s = r0; s != CB_NONE32 && alive; s = chain_next(t, s, CB_SCOPE_FLAG_RESOURCE)) {
-        const uint32_t bid = ldg(t.res_block_map() + bm_base + s);
-        if (bid != CB_NONE32) {
-            const U4 bl = ld16(t.blocks() + bid);   // {row_start, n_rows, DENY rows, -}
-            uint32_t D = 0, A = 0;                  // DENY / ALLOW pair masks of this scope
-            uint32_t ri = bl.x;
+    const U4 *chain = t.uc_chain() + bm_base;
+    for (uint32_t s = r0; s != CB_NONE32 && alive;) {
+        const U4 d = ld16(chain + s);   // {first DENY row, first ALLOW row, end of the ALLOW rows, next scope}
+        uint32_t D = 0, A = 0;          // DENY / ALLOW pair masks of this scope
+        uint32_t ri = d.x;
 #if defined(__CUDA_ARCH__)
 #pragma unroll 1
 #endif
-            for (const uint32_t re = bl.x + bl.z; ri < re; ri++) D |= uc_row_pairs<RP, kForm>(rows.get(aset_base, ri), rp, val, role_all) & alive;
-            alive &= ~D;
+        for (; ri < d.y; ri++) D |= uc_row_pairs<RP, kForm>(rows.get(aset_base, ri), rp, val, role_all) & alive;
+        alive &= ~D;
 #if defined(__CUDA_ARCH__)
 #pragma unroll 4
 #endif
-            for (const uint32_t re = bl.x + bl.y; ri < re; ri++) A |= uc_row_pairs<RP, kForm>(rows.get(aset_base, ri), rp, val, role_all) & alive;
-            if (((ldg(t.scope_flags() + s) >> CB_SCOPE_PERM_SHIFT) & 3) == 1) { allow_pairs |= A; alive &= ~A; }
-        }
+        for (; ri < d.z; ri++) A |= uc_row_pairs<RP, kForm>(rows.get(aset_base, ri), rp, val, role_all) & alive;
+        allow_pairs |= A;   // ALLOW rows are listed only where they count (SCOPE_PERM)
+        alive &= ~A;
+        s = d.w;
     }
     return allow_pairs;
 }
@@ -3496,7 +3501,11 @@ CB_HD bool eval_request_uc(const TableView t, const BatchView &b, const Cols &co
     if (pv != rv) return true;   // existence checks matter only then (ruletable.go:852-863): general body
     uint32_t acc = 0;
     const bool live = n_roles != 0 && K != 0 && rv != CB_NONE16 && kc != CB_KIND_NONE;
+#ifdef CB_UC_STUB_WALK   // tools/uc_variants.sh: no scope chain, no rows (wrong results)
+    const uint32_t r0 = live ? rscope & 0xFFFFu : CB_NONE32;
+#else
     const uint32_t r0 = live ? chain_start(t, rscope, CB_SCOPE_FLAG_RESOURCE, (b.flags & CB_BATCH_FLAG_LENIENT) != 0) : CB_NONE32;
+#endif
     if (r0 != CB_NONE32) {
         bool slow = false;
         const CondWord val = conds(t, b, regs, pid, n, slow);   // bit u: distinct condition u holds; bit 0: "no condition"
@@ -3507,9 +3516,14 @@ CB_HD bool eval_request_uc(const TableView t, const BatchView &b, const Cols &co
         const uint32_t alive0 = amask * role_all;
         const uint32_t bm_base = (rv * t.L->nRP + kc) * t.L->nS;
         uint32_t allow_pairs;
+#ifdef CB_UC_STUB_WALK
+        allow_pairs = alive0 & ((uint32_t)val.lo ^ (uint32_t)(val.lo >> 32) ^ (uint32_t)rp ^ r0 ^ bm_base ^ aset_base);
+        (void)rows;
+#else
         // the role table gets one more field, "any role"; when it all fits 32 bits the per-row shift is a single SHF
-        if ((t.L->nR + 1) * RCP <= 32) allow_pairs = uc_walk<uint32_t, Conds::kForm>(t, b, rows, (uint32_t)rp | role_all << (t.L->nR * RCP), val, r0, bm_base, aset_base, role_all, alive0);
-        else allow_pairs = uc_walk<uint64_t, Conds::kForm>(t, b, rows, rp | (uint64_t)role_all << (t.L->nR * RCP), val, r0, bm_base, aset_base, role_all, alive0);
+        if ((t.L->nR + 1) * RCP <= 32) allow_pairs = uc_walk<uint32_t, Conds::kForm>(t, rows, (uint32_t)rp | role_all << (t.L->nR * RCP), val, r0, bm_base, aset_base, role_all, alive0);
+        else allow_pairs = uc_walk<uint64_t, Conds::kForm>(t, rows, rp | (uint64_t)role_all << (t.L->nR * RCP), val, r0, bm_base, aset_base, role_all, alive0);
+#endif
         // fold: an action is ALLOWed iff some role column allowed it; then pack the stride-RC bits
         uint32_t x = allow_pairs;
         x |= RC > 1 ? allow_pairs >> 1 : 0u;

@@ -513,6 +513,20 @@ inline UcSource generate_uc(const uint8_t *uc_image, const uint32_t *off, uint32
     uint32_t n_pred_bits = (uint32_t)pred_terms.size();
     for (uint32_t a = 0; a < atoms.src.size(); a++)
         if (atoms.only_slot[a] != CB_NONE32 && !atoms.reads_pid[a] && n_pred_bits + 2 <= 32) { atom_pred[a] = (int)n_pred_bits; n_pred_bits += 2; }
+    // set predicates over two slot lists share one membership mask per list pair (cb_core.h: list_mask): isSubset(A, B)
+    // needs "which elements of A occur in B", hasIntersection over the pair takes whichever orientation exists
+    std::map<std::pair<uint32_t, uint32_t>, bool> masks;   // (A, B) -> emitted
+    std::vector<std::pair<uint32_t, uint32_t>> mask_of(terms.size());
+    for (int pass = 0; pass < 2; pass++)
+        for (uint32_t q = 0; q < terms.size(); q++) {
+            const uint32_t *w = terms[q].data();
+            const uint32_t op = w[0] & 0xFF;
+            if (form[q] != 'L' || (op != CB_TERM_SUBSET && op != CB_TERM_INTERSECTS) || (op == CB_TERM_SUBSET) != (pass == 0)) continue;
+            std::pair<uint32_t, uint32_t> k(w[1], w[2]);
+            if (op == CB_TERM_INTERSECTS && !masks.count(k) && masks.count({w[2], w[1]})) k = {w[2], w[1]};
+            masks[k] = true;
+            mask_of[q] = k;
+        }
     auto sl = [](uint32_t v) { return "cols.slot(" + std::to_string(v) + "u)"; };
     auto term_code = [&](uint32_t q) -> std::string {
         const uint32_t *w = terms[q].data();
@@ -523,7 +537,8 @@ inline UcSource generate_uc(const uint8_t *uc_image, const uint32_t *off, uint32
             if (op == CB_TERM_IN_SS) return "list_in_tri(" + sl(w[1]) + ", cols.l" + std::to_string(w[2]) + ", slow)";
             if (op == CB_TERM_IN)
                 return "list_in_tri(term_operand(t, b, cols, pid, " + hex(xk) + ", " + hex(w[1]) + ", " + hex(w[3] & 0xFFFFu) + "), cols.l" + std::to_string(w[2]) + ", slow)";
-            return std::string("list_set_tri(") + (op == CB_TERM_SUBSET ? "true" : "false") + ", cols.l" + std::to_string(w[1]) + ", cols.l" + std::to_string(w[2]) + ", slow)";
+            const std::string a = std::to_string(mask_of[q].first), bb = std::to_string(mask_of[q].second);
+            return std::string("list_set_tri(") + (op == CB_TERM_SUBSET ? "true" : "false") + ", cols.l" + a + ", cols.l" + bb + ", m" + a + "_" + bb + ", slow)";
         }
         return term_expr(w, consts, theap);
     };
@@ -578,6 +593,10 @@ inline UcSource generate_uc(const uint8_t *uc_image, const uint32_t *off, uint32
     }
     s += "        (void)slow; (void)pid;\n        return bits;\n    }\n";
     s += "    CB_HD CondWord operator()(const TableView t, const BatchView &b, const SpecRegs &cols, uint32_t pid, uint64_t n, bool &slow) const {\n";
+    for (const auto &m : masks) {
+        const std::string a = std::to_string(m.first.first), bb = std::to_string(m.first.second);
+        s += "        const uint32_t m" + a + "_" + bb + " = list_mask(cols.l" + a + ", cols.l" + bb + ");   // elements of slot " + a + " in slot " + bb + "\n";
+    }
     for (uint32_t q = 0; q < terms.size(); q++)
         s += "        const int q" + std::to_string(q) + " = " + term_code(q) + ";\n";
     if (have_atoms) {

@@ -105,6 +105,42 @@ inline Image build(const uint8_t *image, const uint32_t *off, const uint64_t *le
         ublocks[4 * b + 2] = n_deny;
         ublocks[4 * b + 3] = 0;
     }
+    // Chain descriptors: one step record per RES_BLOCK_MAP entry (version, kind pattern, scope s), so that the walk
+    // (cb::uc_walk) reads one record per scope instead of the block map, the block, the scope flags and the parent chain:
+    //   {first DENY row, first ALLOW row, end of the ALLOW rows, next scope of the resource chain (chain_next; CB_NONE32)}
+    // A scope whose ALLOWs do not count (SCOPE_PERM != 1) lists no ALLOW rows: the walk applies a scope's ALLOW mask
+    // only where they count, so those rows can never change a result.  Not lenient-dependent: only the chain's first
+    // scope is (chain_start, per request).
+    const uint32_t nS = meta[CB_META_N_SCOPES];
+    const uint64_t n_map = (uint64_t)meta[CB_META_N_VERSIONS] * meta[CB_META_N_RESPATS] * nS;
+    if (nS == 0 || len[CB_SEC_SCOPE_PARENT] < (uint64_t)nS * 4 || len[CB_SEC_SCOPE_FLAGS] < (uint64_t)nS * 4 || len[CB_SEC_RES_BLOCK_MAP] < n_map * 4) {
+        out.why = "scope tables do not match the block map";
+        return out;
+    }
+    const uint32_t *parent = reinterpret_cast<const uint32_t *>(image + off[CB_SEC_SCOPE_PARENT]);
+    const uint32_t *sflags = reinterpret_cast<const uint32_t *>(image + off[CB_SEC_SCOPE_FLAGS]);
+    const uint32_t *bmap = reinterpret_cast<const uint32_t *>(image + off[CB_SEC_RES_BLOCK_MAP]);
+    std::vector<uint32_t> next(nS);
+    for (uint32_t s = 0; s < nS; s++) {
+        uint32_t x = s, steps = 0;
+        do { x = parent[x]; } while (x != CB_NONE32 && x < nS && ++steps <= nS && !(sflags[x] & CB_SCOPE_FLAG_RESOURCE));
+        if (x != CB_NONE32 && (x >= nS || steps > nS)) { out.why = "scope parent chain out of range"; return out; }
+        next[s] = x;
+    }
+    std::vector<uint32_t> chain(4 * (size_t)n_map, 0);
+    for (uint64_t e = 0; e < n_map; e++) {
+        const uint32_t s = (uint32_t)(e % nS), bid = bmap[e];
+        uint32_t *d = chain.data() + 4 * e;
+        if (bid != CB_NONE32) {
+            if (bid >= n_blocks) { out.why = "block map entry out of range"; return out; }
+            const uint32_t *bl = ublocks.data() + 4 * (size_t)bid;   // {row_start, n_rows, DENY rows, 0}
+            const bool allow_counts = ((sflags[s] >> CB_SCOPE_PERM_SHIFT) & 3) == 1;
+            d[0] = bl[0];
+            d[1] = bl[0] + bl[2];
+            d[2] = allow_counts ? bl[0] + bl[1] : d[1];
+        }
+        d[3] = next[s];
+    }
     // compact image: the sections the unique-condition kernels (and the interpreter they may call) read
     out.lay = lay;
     for (auto &o : out.lay.off) o = 0;
@@ -115,12 +151,13 @@ inline Image build(const uint8_t *image, const uint32_t *off, const uint64_t *le
         return at;
     };
     append("CBUC", 4);   // offset 0 stays unused: a zero offset means "section not present"
-    out.lay.off[CB_SEC_BLOCKS] = append(ublocks.data(), ublocks.size() * 4);
-    for (int id : {CB_SEC_SCOPE_PARENT, CB_SEC_SCOPE_FLAGS, CB_SEC_RES_BLOCK_MAP, CB_SEC_CODE, CB_SEC_CONSTS, CB_SEC_CONSTS_V64, CB_SEC_THEAP,
+    // (the blocks and the block map are folded into the chain descriptors)
+    for (int id : {CB_SEC_SCOPE_PARENT, CB_SEC_SCOPE_FLAGS, CB_SEC_CODE, CB_SEC_CONSTS, CB_SEC_CONSTS_V64, CB_SEC_THEAP,
                    CB_SEC_STR_OFF, CB_SEC_STR_BYTES})
         out.lay.off[id] = append(image + off[id], len[id]);
     out.lay.uc_conds_off = append(ucond_rec.data(), ucond_rec.size() * 4);
     out.lay.uc_rows_off = append(urows.data(), urows.size() * 4);
+    out.lay.uc_chain_off = append(chain.data(), chain.size() * 4);
     out.lay.n_uconds = out.n_uconds;
     out.lay.theap_words = (uint32_t)(len[CB_SEC_THEAP] / 8);
     out.lay.image_bytes = (uint32_t)out.bytes.size();

@@ -707,8 +707,10 @@ SpecForm spec_compile(const uint8_t *image, const cb::TableLayout &lay, const ui
     const char *mb = getenv("CERBOS_B200_SPEC_BLOCKS");   // experiments: resident CTAs / SM the specialised kernels are budgeted for
     const std::string mbopt = std::string("-DCB_SPEC_MIN_BLOCKS=") + (mb && mb[0] >= '1' && mb[0] <= '8' && !mb[1] ? mb : "5");
     const char *ub = getenv("CERBOS_B200_SPEC_UC_BLOCKS");
-    // leaf programs keep whole values (tag + payload) in registers: budget 128 registers / thread for them, 64 otherwise
-    const std::string ubopt = std::string("-DCB_SPEC_UC_MIN_BLOCKS=") + (ub && ub[0] >= '1' && ub[0] <= '8' && !ub[1] ? ub : n_atoms ? "2" : "4");
+    // leaf programs keep whole values (tag + payload) in registers: budget 128 registers / thread for them, 80 otherwise
+    // (at 64, C3's register-resident slots and lists spill to local memory; on an H100, 3 CTAs / SM at 80 registers run
+    // C3 in 2.28 ms per 2^24 batch against 3.03 ms at 4 CTAs / SM)
+    const std::string ubopt = std::string("-DCB_SPEC_UC_MIN_BLOCKS=") + (ub && ub[0] >= '1' && ub[0] <= '8' && !ub[1] ? ub : n_atoms ? "2" : "3");
     if (const char *dump = getenv("CERBOS_B200_SPEC_DUMP")) {   // profiling aid: the translation unit handed to NVRTC
         if (FILE *f = fopen(dump, "w")) { fwrite(src.data(), 1, src.size(), f); fclose(f); }
     }

@@ -1,8 +1,10 @@
 #!/bin/bash
 # Times the C3 check kernel under experiment switches of the run-time specialised build (one bench.py run per variant;
 # kernel_ms_mean = CUDA events around the check kernel alone).  Usage (needs a GPU): tools/uc_variants.sh [requests]
+# The stub_* variants replace one phase of cb::eval_request_uc by a trivial stand-in whose result is still stored
+# (cb_core.h: CB_UC_STUB_*; their decisions are wrong, hence --no-verify): default minus stub = that phase's share.
 OUT=${OUT:-profile_out}; mkdir -p "$OUT"
-N=${1:-4194304}
+N=${1:-16777216}
 out=$OUT/uc_variants.txt
 : > "$out"
 run() {
@@ -11,7 +13,10 @@ run() {
     echo "$name $(echo "$line" | python -c 'import sys,json; d=json.load(sys.stdin); r=d["roofline"]; print(r["kernel_ms_mean"], r["frac"], d["config"]["kernel"]["grid"])' 2>&1)" | tee -a $out
 }
 run default X=1
+run stub_walk CERBOS_B200_SPEC_DEFS=-DCB_UC_STUB_WALK
+run stub_lists CERBOS_B200_SPEC_DEFS=-DCB_UC_STUB_LISTS
+run stub_strpred CERBOS_B200_SPEC_DEFS=-DCB_UC_STUB_STRPRED
 run keys64 CERBOS_B200_SPEC_DEFS=-DCB_LIST_KEYS64
 run blocks3 CERBOS_B200_SPEC_UC_BLOCKS=3
+run blocks4 CERBOS_B200_SPEC_UC_BLOCKS=4
 run blocks5 CERBOS_B200_SPEC_UC_BLOCKS=5
-run blocks6 CERBOS_B200_SPEC_UC_BLOCKS=6

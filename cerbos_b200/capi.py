@@ -16,7 +16,7 @@ OK, ERR_INVALID, ERR_CUDA, ERR_UNSUPPORTED, ERR_NO_DEVICE = 0, -1, -2, -3, -4
 
 EXPORTS = [
     "cgpu_init", "cgpu_shutdown", "cgpu_table_load", "cgpu_table_retain", "cgpu_table_release", "cgpu_check", "cgpu_check_meta", "cgpu_check_narrow",
-    "cgpu_check_device", "cgpu_sync", "cgpu_launch_count", "cgpu_table_info", "cgpu_last_kernel_config",
+    "cgpu_check_device", "cgpu_sync", "cgpu_launch_count", "cgpu_deferred_count", "cgpu_table_info", "cgpu_last_kernel_config",
     "cgpu_last_cluster_config", "cgpu_profile", "cgpu_table_wait_ready", "cgpu_table_compile_check", "cgpu_peer_alloc", "cgpu_peer_open", "cgpu_peer_close",
     "cgpu_peer_free", "cgpu_peer_read", "cgpu_check_device_gather", "cgpu_gather_wait", "cgpu_last_error",
     "cgpu_device_count", "cgpu_encoder_create", "cgpu_encoder_destroy", "cgpu_encode", "cgpu_encoded_batch", "cgpu_encoded_free",
@@ -84,6 +84,8 @@ def lib():
         L.cgpu_sync.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
         L.cgpu_launch_count.restype = ctypes.c_uint64
         L.cgpu_launch_count.argtypes = [ctypes.c_void_p]
+        L.cgpu_deferred_count.restype = ctypes.c_int
+        L.cgpu_deferred_count.argtypes = [ctypes.c_void_p, ctypes.POINTER(ctypes.c_uint64)]
         L.cgpu_table_info.restype = ctypes.c_int
         L.cgpu_table_info.argtypes = [ctypes.c_void_p, ctypes.POINTER(ctypes.c_uint32), ctypes.c_uint32]
         L.cgpu_last_kernel_config.restype = ctypes.c_int
@@ -236,6 +238,12 @@ class Context:
 
     def launch_count(self) -> int:
         return int(lib().cgpu_launch_count(self._h))
+
+    def deferred_count(self) -> int:
+        """requests the lean / unique-condition kernels left to the general kernel so far (synchronises)"""
+        n = ctypes.c_uint64()
+        _check(lib().cgpu_deferred_count(self._h, ctypes.byref(n)))
+        return n.value
 
     def last_kernel_config(self):
         g, b, s = ctypes.c_uint32(), ctypes.c_uint32(), ctypes.c_uint32()

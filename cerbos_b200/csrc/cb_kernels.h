@@ -103,6 +103,8 @@ __device__ __forceinline__ void check_body(const TableDesc &td, const cb::BatchV
         if (bv.count_dev && bv.sig_step && blockIdx.x == 0 && threadIdx.x < 32) gather_signal_flags(bv);
         return;
     }
+    // the cell's last word keeps a running total of the requests drained through it (cgpu_deferred_count)
+    if (bv.count_dev && blockIdx.x == 0 && threadIdx.x == 0) bv.count_dev[3] += (uint32_t)count;
     const uint8_t *base = td.base;
     if (kStage) {
         if (threadIdx.x == 0) {

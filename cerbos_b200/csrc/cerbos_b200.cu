@@ -362,7 +362,7 @@ struct cgpu_ctx {
         uint32_t seq = 0;
         uint32_t *lists[4] = {nullptr, nullptr, nullptr, nullptr};
         size_t cap[4] = {0, 0, 0, 0};
-        uint32_t *cells = nullptr;   // 4 x {count, done, tile counter, -}, zero between uses (the drain kernel re-zeroes)
+        uint32_t *cells = nullptr;   // 4 x {count, done, tile counter, drained total}, count / done zero between uses (the drain kernel re-zeroes)
         uint32_t *strpred[4] = {nullptr, nullptr, nullptr, nullptr};   // per-string predicate words of the specialised unique-condition kernels
         size_t sp_cap[4] = {0, 0, 0, 0};
         cb::U4 *pk[4] = {nullptr, nullptr, nullptr, nullptr};          // merged row records of unique-condition launches on a global image
@@ -869,7 +869,7 @@ int acquire_defer(cgpu_ctx *ctx, cudaStream_t stream, uint64_t count, uint32_t *
         *pk = ln.pk[q];
     }
     *list = ln.lists[q];
-    *cell = ln.cells + 4 * q;   // {count, done, tile counter, -}
+    *cell = ln.cells + 4 * q;   // {count, done, tile counter, drained total}
     return CGPU_OK;
 }
 
@@ -1254,6 +1254,30 @@ int cgpu_table_info(const cgpu_table *t, uint32_t *meta_out, uint32_t n_words) {
 }
 
 uint64_t cgpu_launch_count(const cgpu_ctx *ctx) { return ctx ? ctx->launches.load() : 0; }
+
+int cgpu_deferred_count(cgpu_ctx *ctx, uint64_t *total) {
+    if (!ctx || !total) return fail(CGPU_ERR_INVALID, "cgpu_deferred_count: null argument");
+    *total = 0;
+    struct RestoreDevice {   // the caller's current device, whichever way this returns
+        int dev = -1;
+        RestoreDevice() { if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); dev = -1; } }
+        ~RestoreDevice() { if (dev >= 0) cudaSetDevice(dev); }
+    } restore;
+    std::vector<cgpu_ctx *> all{ctx};
+    all.insert(all.end(), ctx->peers.begin(), ctx->peers.end());
+    for (cgpu_ctx *c : all) {
+        CUDA_TRY(cudaSetDevice(c->device));
+        CUDA_TRY(cudaDeviceSynchronize());
+        std::lock_guard<std::mutex> g(c->defer_mu);
+        for (auto &kv : c->defer_lanes) {
+            if (!kv.second.cells) continue;
+            uint32_t w[16];
+            CUDA_TRY(cudaMemcpy(w, kv.second.cells, sizeof(w), cudaMemcpyDeviceToHost));
+            for (int q = 0; q < 4; q++) *total += w[4 * q + 3];
+        }
+    }
+    return CGPU_OK;
+}
 
 int cgpu_last_kernel_config(const cgpu_ctx *ctx, uint32_t *grid, uint32_t *block, uint32_t *smem_bytes) {
     if (!ctx) return fail(CGPU_ERR_INVALID, "null ctx");

@@ -233,6 +233,11 @@ int cgpu_gather_wait(cgpu_ctx *ctx, const uint32_t *local_flags, uint32_t n_rank
 
 /* Introspection used by bench.py / tests (not part of the Go surface). */
 uint64_t cgpu_launch_count(const cgpu_ctx *ctx);        /* kernels launched by this library so far */
+/* Test aid: requests the lean and unique-condition kernels have left to the general kernel so far, summed over every
+ * stream of the context and its peer devices.  Each deferral-counter cell keeps a 32-bit running total, which wraps after
+ * 2^32 deferrals through that cell: compare differences over a few launches, not lifetime totals.  Synchronises the
+ * devices; the calling thread's current device is left as it was. */
+int cgpu_deferred_count(cgpu_ctx *ctx, uint64_t *total);
 int cgpu_table_info(const cgpu_table *t, uint32_t *meta_out, uint32_t n_words);  /* copies META words */
 int cgpu_last_kernel_config(const cgpu_ctx *ctx, uint32_t *grid, uint32_t *block, uint32_t *smem_bytes);
 /* Whether the last launch evaluated in clustered order (requests grouped by policy block inside L2-sized windows by

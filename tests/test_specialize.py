@@ -9,6 +9,7 @@ import pytest
 import workloads as W
 from cerbos_b200.encode import Encoder
 from cerbos_b200.policy.compile import build_rule_table
+from cerbos_b200.table import layout as L
 from cerbos_b200.table.flatten import flatten
 from fuzzgen import rand_policies, rand_request
 from hostsim import driver as hostsim
@@ -120,29 +121,31 @@ def test_unique_condition_body_on_random_tables(seed, tmp_path):
     docs = [d for d in rand_policies(r) if "resourcePolicy" in d or "derivedRoles" in d or "exportVariables" in d or "exportConstants" in d]
     rt = build_rule_table(docs)
     ft = flatten(rt)
-    enc = Encoder(ft.manifest)
+    lenient = seed % 4 == 0
+    fl = L.BATCH_FLAG_LENIENT if lenient else 0
+    enc = Encoder(ft.manifest, lenient_scope_search=lenient)
     inputs = [rand_request(r) for _ in range(300)]
     b = enc.encode(inputs)
     try:
-        want = cref.check(ft.blob, b.columns, b.n, b.max_actions, 0, 0)
+        want = cref.check(ft.blob, b.columns, b.n, b.max_actions, 0, fl)
     except RuntimeError as e:
         if "-2" in str(e):
             pytest.skip("a request produces a run-time value outside the device's exact range (oracle #2 flags it too)")
         raise
     valid = want != 0
     try:
-        got = hostsim.check(ft.blob, b.columns, b.n, b.max_actions, mode=4)
+        got = hostsim.check(ft.blob, b.columns, b.n, b.max_actions, 0, fl, mode=4)
     except RuntimeError as e:
         if "-3" in str(e):
             pytest.skip("no unique-condition image (too many distinct conditions)")
         raise
     assert (got[valid] == want[valid]).all(), seed
-    got = hostsim.check(ft.blob, b.columns, b.n, b.max_actions, mode=5)
+    got = hostsim.check(ft.blob, b.columns, b.n, b.max_actions, 0, fl, mode=5)
     assert (got[valid] == want[valid]).all(), seed
     src, nu = hostsim.generate_uc(ft.blob)
     if src:
         lib = hostsim.build_spec(ft.blob, str(tmp_path), uc=True)
-        got = hostsim.check_spec(lib, ft.blob, b.columns, b.n, b.max_actions, mode=5)
+        got = hostsim.check_spec(lib, ft.blob, b.columns, b.n, b.max_actions, 0, fl, mode=5)
         assert (got[valid] == want[valid]).all(), seed
 
 

@@ -337,6 +337,54 @@ struct Slot {   // per in-flight cgpu_check call
     bool busy = false;
 };
 
+// The main kernel of a check launch (plan_launch picks it, kernel_fn maps it to its entry point).  The kernels from
+// SpecTiles on are compiled for the table at run time (NVRTC, cb_specialize.h).
+enum class Kernel : uint8_t {
+    General, GeneralGlobal,         // check_kernel<false, 2>: general body, table image staged / read from global memory
+    Lean, LeanGlobal, LeanTiles,    // check_kernel<true, 1> / <true, 0>, check_kernel_tiles (request columns through TMA)
+    Uc, UcGlobal,                   // check_uc<true> / <false>
+    SpecTiles, SpecDirect,          // cb_spec_tiles / cb_spec_direct (block-shape form)
+    SpecUc, SpecUcGlobal,           // cb_spec_uc / cb_spec_uc_global (unique-condition form)
+};
+constexpr int kKernels = (int)Kernel::SpecUcGlobal + 1;
+
+// What one check launch runs: plan_launch decides it, launch_check executes it.
+struct LaunchPlan {
+    Kernel kernel = Kernel::General;
+    uint32_t smem = 0;          // dynamic shared memory of the main kernel
+    uint32_t last_arg = 0;      // its last argument: stage_rt (check_kernel, cb_spec_direct) or n_slots (column tiles)
+    bool stage = false;         // the table image is staged in shared memory (general and lean bodies)
+    bool lean = false;          // lean body: the requests it defers go to a list the general kernel drains right behind it
+    bool uc = false;            // unique-condition kernel
+    bool uc_staged = false;     // ... with its compact image and merged rows in shared memory
+    bool col_tiles = false;     // request columns staged tile by tile through TMA
+    bool cluster = false;       // clustered evaluation order
+    bool spec = false;          // the kernel compiled for this table at run time
+    bool strpred = false;       // the kernel reads per-string predicate words (filled by cb_spec_strpred)
+    bool merge_rows = false;    // uc_merge_rows pre-pass
+    bool serialise = false;     // programmatically serialised behind the previous launch's drain kernel
+};
+
+// A device buffer of a deferral lane.  fit() grows it to a power of two of at least min_cap elements, stream-ordered: the
+// old buffer is released only after everything queued on this stream so far -- the only launches that can still read
+// it -- has completed.
+template <class T> struct LaneBuf {
+    T *ptr = nullptr;
+    size_t cap = 0;
+    cudaError_t fit(size_t n, size_t min_cap, cudaStream_t stream) {
+        if (cap >= n) return cudaSuccess;
+        size_t c = min_cap;
+        while (c < n) c <<= 1;
+        T *fresh = nullptr;
+        const cudaError_t e = cudaMallocAsync(reinterpret_cast<void **>(&fresh), c * sizeof(T), stream);
+        if (e != cudaSuccess) return e;
+        T *old = ptr;
+        ptr = fresh;
+        cap = c;
+        return old ? cudaFreeAsync(old, stream) : cudaSuccess;
+    }
+};
+
 }  // namespace
 
 struct cgpu_ctx {
@@ -347,26 +395,25 @@ struct cgpu_ctx {
     std::atomic<uint64_t> launches{0};
     std::mutex mu;
     std::vector<Slot> slots;
-    uint32_t last_grid = 0, last_block = 0, last_smem = 0, last_fast = 0;
+    // the last check launch (cgpu_last_kernel_config / cgpu_last_cluster_config); window / buckets: the last clustered one
+    LaunchPlan last_plan;
+    uint32_t last_grid = 0, last_window = 0, last_buckets = 0;
     int force_no_stage = 0;
     int force_general = 0;   // CERBOS_B200_FORCE_GENERAL=1: never pick the lean kernel body (tests)
     int cluster_mode = -1;   // CERBOS_B200_CLUSTER: 0 never, 1 always, unset = batches of >= kClusterMinRequests
-    uint32_t last_clustered = 0, last_window = 0, last_buckets = 0, last_col_tiles = 0;
     int force_no_tiles = 0;  // CERBOS_B200_NO_TILES=1: never stage request columns through TMA (tests)
     int force_no_jit = 0;    // CERBOS_B200_NO_JIT=1: never compile table-specialised kernels (tests)
-    uint32_t last_spec = 0;
     // Deferral state is owned by the STREAM a launch is issued on (a cgpu_check slot has its own stream): launches on one
     // stream complete in order, and with programmatic launch chaining at most three consecutive ones are in flight
     // together (k draining, k+1 running, k+2 starting), so every stream rotates over four lists / counter cells of its own.
     struct DeferLane {
         uint32_t seq = 0;
-        uint32_t *lists[4] = {nullptr, nullptr, nullptr, nullptr};
-        size_t cap[4] = {0, 0, 0, 0};
         uint32_t *cells = nullptr;   // 4 x {count, done, tile counter, drained total}, count / done zero between uses (the drain kernel re-zeroes)
-        uint32_t *strpred[4] = {nullptr, nullptr, nullptr, nullptr};   // per-string predicate words of the specialised unique-condition kernels
-        size_t sp_cap[4] = {0, 0, 0, 0};
-        cb::U4 *pk[4] = {nullptr, nullptr, nullptr, nullptr};          // merged row records of unique-condition launches on a global image
-        size_t pk_cap[4] = {0, 0, 0, 0};
+        struct Bufs {
+            LaneBuf<uint32_t> list;
+            LaneBuf<uint32_t> strpred;   // per-string predicate words of the specialised unique-condition kernels
+            LaneBuf<cb::U4> pk;          // merged row records of unique-condition launches on a global image
+        } q[4];
     };
     std::map<cudaStream_t, DeferLane> defer_lanes;
     std::mutex defer_mu;
@@ -380,7 +427,6 @@ struct cgpu_ctx {
     std::mutex meta_mu;      // cgpu_check_meta calls share ctx->stream
     std::vector<cgpu_ctx *> peers;   // cgpu_init with n_devices > 1: the contexts of devices 1..n-1 (owned)
     int uc_mode = -1;        // CERBOS_B200_UC: 0 never use the unique-condition kernels, 1 whenever the table allows, unset = tables with > 1 block shape
-    uint32_t last_uc = 0;
     bool profiling = false;  // cgpu_profile(): CUDA events around the check kernel of every launch
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     double prof_ms = 0;
@@ -417,8 +463,8 @@ struct cgpu_table {
     uint8_t *d_image = nullptr;
     TableDesc desc{};
     uint32_t meta[CB_META_WORDS]{};
-    std::atomic<int> occ[11]{};
-    std::atomic<uint32_t> occ_smem[11]{};
+    // resident CTAs / SM per kernel (resident_ctas): footprint << 32 | CTAs in one word, 0 = not queried yet
+    mutable std::atomic<uint64_t> occ[kKernels]{};
     // table-specialised lean kernels (cb_specialize.h), compiled with NVRTC on first use
     std::vector<uint8_t> host_image;
     std::mutex spec_mu;
@@ -434,7 +480,7 @@ struct cgpu_table {
     uint8_t *d_uc_image = nullptr;
     TableDesc uc_desc{};
     std::thread spec_thread;          // compiles the specialised kernels in the background from cgpu_table_load on
-    std::mutex join_mu;   // resident CTAs / SM per kernel variant (0 = not queried yet)
+    std::mutex join_mu;
 };
 
 namespace {
@@ -659,12 +705,24 @@ void cache_write(const std::string &path, const std::vector<char> &data) {
 // unique-condition form when every distinct condition has a flat form.  `gen` receives the generated source.
 enum SpecForm { SPEC_NONE = 0, SPEC_SHAPES = 1, SPEC_UC = 2 };
 constexpr uint32_t kUcMaxSmem = 72 * 1024;   // compact image + merged rows: three CTAs / SM at least
+
+// Resource-policy-only tables (no principal / role policies, no parent roles) whose kinds resolve without resource globs:
+// the only tables a lean kernel body can evaluate.
+bool lean_table(const cb::TableLayout &lay, const uint32_t *meta) {
+    return !lay.has_principal_policies && !lay.has_role_policies && !lay.has_parent_roles && meta[CB_META_DIRECT_KINDS];
+}
+// Shared memory of a staged unique-condition launch: the compact image, then one 16-byte merged row per (action set, row).
+uint64_t uc_smem_bytes(const cbuc::Image &uc, uint64_t n_pk) { return (((uint64_t)uc.lay.image_bytes + 127) & ~127ull) + 16 * n_pk; }
+// Whether the staged unique-condition kernel fits with n_pk merged rows.  With one (the default) it is the question whether
+// the image leaves room at all, which decides whether the specialised translation unit carries the staged kernel.
+bool uc_stageable(const cbuc::Image &uc, uint64_t n_pk = 1) { return uc_smem_bytes(uc, n_pk) <= kUcMaxSmem; }
+
 SpecForm spec_generate(const uint8_t *image, const cb::TableLayout &lay, const uint32_t *meta, const cbuc::Image &uc, std::string *gen, std::string *why, uint32_t *n_strpred,
                        uint32_t *n_atoms = nullptr) {
     *n_strpred = 0;
     if (n_atoms) *n_atoms = 0;
-    // the specialised kernels are lean bodies: a table launch_check can never route to a lean kernel needs none
-    if (lay.has_principal_policies || lay.has_role_policies || lay.has_parent_roles || !meta[CB_META_DIRECT_KINDS]) {
+    // the specialised kernels are lean bodies: a table that can never take a lean kernel needs none
+    if (!lean_table(lay, meta)) {
         *why = "table is not lean-eligible (principal / role policies, parent roles or resource globs): general kernel only";
         return SPEC_NONE;
     }
@@ -700,7 +758,7 @@ SpecForm spec_compile(const uint8_t *image, const cb::TableLayout &lay, const ui
     if (form == SPEC_UC) {
         // an image that can never be staged (larger than the shared-memory budget of the staged kernel) gets the global
         // variant only, a small one both: which of the two a launch takes also depends on the batch's action sets
-        if (uc.lay.image_bytes + 128u <= kUcMaxSmem) src += kSpecUcStaged;
+        if (uc_stageable(uc)) src += kSpecUcStaged;
         src += kSpecUcGlobal;
         src += kSpecUcStrpred;
     } else src += kSpecKernels;
@@ -766,8 +824,7 @@ bool ensure_spec(cgpu_ctx *ctx, cgpu_table *t) {
     const SpecForm form = spec_compile(t->host_image.data(), t->desc.lay, t->meta, t->uc, &cubin, &why, &t->spec_n_strpred);
     if (form == SPEC_NONE) return give_up(why);
     if (cudaLibraryLoadData(&t->spec_lib, cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0) != cudaSuccess) { cudaGetLastError(); return give_up("cudaLibraryLoadData failed"); }
-    const bool staged_variant = t->uc.lay.image_bytes + 128u <= kUcMaxSmem;
-    bool got = form == SPEC_UC ? (!staged_variant || cudaLibraryGetKernel(&t->spec_uc, t->spec_lib, "cb_spec_uc") == cudaSuccess) &&
+    bool got = form == SPEC_UC ? (!uc_stageable(t->uc) || cudaLibraryGetKernel(&t->spec_uc, t->spec_lib, "cb_spec_uc") == cudaSuccess) &&
                                      cudaLibraryGetKernel(&t->spec_uc_global, t->spec_lib, "cb_spec_uc_global") == cudaSuccess &&
                                      cudaLibraryGetKernel(&t->spec_strpred, t->spec_lib, "cb_spec_strpred") == cudaSuccess
                                : cudaLibraryGetKernel(&t->spec_tiles, t->spec_lib, "cb_spec_tiles") == cudaSuccess &&
@@ -823,9 +880,10 @@ int launch_cluster(cgpu_ctx *ctx, const cgpu_table *t, const cb::BatchView &bv, 
     return CGPU_OK;
 }
 
-// The launch's deferral list + counter cell, owned by the stream it is issued on (see cgpu_ctx::DeferLane).
-int acquire_defer(cgpu_ctx *ctx, cudaStream_t stream, uint64_t count, uint32_t **list, uint32_t **cell, size_t n_strpred = 0, uint32_t **strpred = nullptr,
-                  size_t n_pk = 0, cb::U4 **pk = nullptr) {
+// The launch's deferral list + counter cell, and the pre-pass buffers it asks for (n_strpred / n_pk elements; 0: none,
+// the pointer is then null), owned by the stream it is issued on (see cgpu_ctx::DeferLane).
+int acquire_defer(cgpu_ctx *ctx, cudaStream_t stream, uint64_t count, uint32_t **list, uint32_t **cell, size_t n_strpred, uint32_t **strpred,
+                  size_t n_pk, cb::U4 **pk) {
     std::lock_guard<std::mutex> g(ctx->defer_mu);
     cgpu_ctx::DeferLane &ln = ctx->defer_lanes[stream];
     if (!ln.cells) {
@@ -833,147 +891,161 @@ int acquire_defer(cgpu_ctx *ctx, cudaStream_t stream, uint64_t count, uint32_t *
         CUDA_TRY(cudaMemset(ln.cells, 0, 4 * 16));
     }
     const uint32_t q = ln.seq++ & 3;
-    if (ln.cap[q] < (size_t)count) {
-        // grow (power-of-two capacities), stream-ordered: the old list is released only after everything queued on this
-        // stream so far -- the only launches that can still read it -- has completed
-        size_t cap = 1024;
-        while (cap < (size_t)count) cap <<= 1;
-        uint32_t *fresh = nullptr;
-        CUDA_TRY(cudaMallocAsync(reinterpret_cast<void **>(&fresh), cap * 4, stream));
-        if (ln.lists[q]) CUDA_TRY(cudaFreeAsync(ln.lists[q], stream));
-        ln.lists[q] = fresh;
-        ln.cap[q] = cap;
-    }
-    if (strpred) {
-        if (ln.sp_cap[q] < n_strpred) {
-            size_t cap = 4096;
-            while (cap < n_strpred) cap <<= 1;
-            uint32_t *fresh = nullptr;
-            CUDA_TRY(cudaMallocAsync(reinterpret_cast<void **>(&fresh), cap * 4, stream));
-            if (ln.strpred[q]) CUDA_TRY(cudaFreeAsync(ln.strpred[q], stream));
-            ln.strpred[q] = fresh;
-            ln.sp_cap[q] = cap;
-        }
-        *strpred = ln.strpred[q];
-    }
-    if (pk) {
-        if (ln.pk_cap[q] < n_pk) {
-            size_t cap = 4096;
-            while (cap < n_pk) cap <<= 1;
-            cb::U4 *fresh = nullptr;
-            CUDA_TRY(cudaMallocAsync(reinterpret_cast<void **>(&fresh), cap * 16, stream));
-            if (ln.pk[q]) CUDA_TRY(cudaFreeAsync(ln.pk[q], stream));
-            ln.pk[q] = fresh;
-            ln.pk_cap[q] = cap;
-        }
-        *pk = ln.pk[q];
-    }
-    *list = ln.lists[q];
+    cgpu_ctx::DeferLane::Bufs &b = ln.q[q];
+    CUDA_TRY(b.list.fit(count, 1024, stream));
+    if (n_strpred) CUDA_TRY(b.strpred.fit(n_strpred, 4096, stream));
+    if (n_pk) CUDA_TRY(b.pk.fit(n_pk, 4096, stream));
+    *list = b.list.ptr;
     *cell = ln.cells + 4 * q;   // {count, done, tile counter, drained total}
+    *strpred = n_strpred ? b.strpred.ptr : nullptr;
+    *pk = n_pk ? b.pk.ptr : nullptr;
     return CGPU_OK;
 }
 
-int launch_check(cgpu_ctx *ctx, const cgpu_table *t, const cb::BatchView &bv, uint8_t *d_bitmap, uint8_t *d_effects,
-                 uint32_t *d_status, cudaStream_t stream, bool *drained = nullptr) {
-    const cb::TableLayout &lay = t->desc.lay;
-    if (drained) *drained = false;
-    const bool stage = !ctx->force_no_stage && lay.image_bytes <= kMaxStageBytes;
-    uint64_t tiles = (bv.count + kThreads - 1) / kThreads;
-    // The lean body applies to resource-policy-only tables (no principal / role policies, parent roles or
-    // resource globs) when the (action x role column) pair masks fit 32 bits and the role table fits 64 bits.
+// Which kernels one check launch runs, and how: from the table, the batch and the context's switches alone (no CUDA call).
+LaunchPlan plan_launch(const cgpu_ctx &ctx, const cgpu_table &t, const cb::BatchView &bv) {
+    const cb::TableLayout &lay = t.desc.lay;
+    LaunchPlan p;
+    p.stage = !ctx.force_no_stage && lay.image_bytes <= kMaxStageBytes;
     uint32_t rcp = 1;
     while (rcp < bv.role_cols) rcp <<= 1;
-    cgpu_table *mt = const_cast<cgpu_table *>(t);
-    const bool uc_spec_ready = mt->spec_state.load(std::memory_order_acquire) == 1 && t->spec_uc_global != nullptr;
+    // the kernels compiled for the table are used once they are loaded: a launch never waits for the compile
+    const bool spec_ready = t.spec_state.load(std::memory_order_acquire) == 1;
+    const bool uc_spec_ready = spec_ready && t.spec_uc_global != nullptr;
     // A table most of whose conditions have no flat form gains nothing from a lean kernel until its specialised kernel
     // (leaf programs as straight-line code) is loaded: the lean body would defer nearly every request to the one-CTA-per-SM
     // drain launch.  Such launches go to the general kernel at full occupancy instead.
-    const bool mostly_programs = t->uc.ok && !uc_spec_ready && 2 * (uint64_t)t->uc.n_gids_flat < t->uc.n_gids;
-    const bool narrow = !ctx->force_general && !mostly_programs && bv.n_pass == 1 && (uint64_t)bv.max_actions * bv.role_cols <= 32 && bv.kbytes <= 4 &&
-                        !lay.has_principal_policies && !lay.has_role_policies && !lay.has_parent_roles &&
-                        t->meta[CB_META_DIRECT_KINDS] && (uint64_t)lay.nR * rcp <= 64;
+    const bool mostly_programs = t.uc.ok && !uc_spec_ready && 2 * (uint64_t)t.uc.n_gids_flat < t.uc.n_gids;
+    // The lean body applies to lean tables when the (action x role column) pair masks fit 32 bits and the role table fits 64 bits.
+    p.lean = !ctx.force_general && !mostly_programs && bv.n_pass == 1 && (uint64_t)bv.max_actions * bv.role_cols <= 32 && bv.kbytes <= 4 &&
+             lean_table(lay, t.meta) && (uint64_t)lay.nR * rcp <= 64;
     // Unique-condition kernels: lean-eligible tables with <= 63 distinct conditions whose blocks differ in shape
     // (with one shape the per-shape specialised tile kernel is the better fit).  Index order, no clustering.
     // (an image with condition programs or index-form rows is only good for the specialised kernel: cbuc::Image::needs_spec)
-    const bool uc = narrow && t->uc.ok && (uc_spec_ready || !t->uc.needs_spec()) && t->d_uc_image && bv.count < (1ull << 32) && (uint64_t)bv.n_asets * lay.n_rows < (1ull << 31) && (uint64_t)(lay.nR + 1) * rcp <= 64 &&
-                    (ctx->uc_mode == 1 || (ctx->uc_mode != 0 && ctx->cluster_mode != 1 && t->meta[CB_META_BLOCK_SHAPES] > 1));   // CERBOS_B200_CLUSTER=1 keeps the clustered path reachable
+    const uint64_t n_pk = (uint64_t)bv.n_asets * lay.n_rows;   // merged rows: one per (action set, row)
+    p.uc = p.lean && t.uc.ok && (uc_spec_ready || !t.uc.needs_spec()) && t.d_uc_image && bv.count < (1ull << 32) && n_pk < (1ull << 31) &&
+           (uint64_t)(lay.nR + 1) * rcp <= 64 &&
+           (ctx.uc_mode == 1 || (ctx.uc_mode != 0 && ctx.cluster_mode != 1 && t.meta[CB_META_BLOCK_SHAPES] > 1));   // CERBOS_B200_CLUSTER=1 keeps the clustered path reachable
     // Clustering pays when the policy blocks differ in shape (rows / conditions): with a single shape every lane runs
     // the same control flow in index order already and the coalesced column loads are worth more.
-    const bool cluster = !uc && bv.count < (1ull << 32) &&
-                         (ctx->cluster_mode == 1 || (ctx->cluster_mode != 0 && bv.count >= kClusterMinRequests && t->meta[CB_META_BLOCK_SHAPES] > 1));
+    p.cluster = !p.uc && bv.count < (1ull << 32) &&
+                (ctx.cluster_mode == 1 || (ctx.cluster_mode != 0 && bv.count >= kClusterMinRequests && t.meta[CB_META_BLOCK_SHAPES] > 1));
     // Index-order lean launches stage the request columns through TMA too, when every tile's column runs are
     // 16-byte aligned and image + two tile stages fit the shared-memory budget of CB_MIN_BLOCKS resident CTAs.
     const uint32_t tile_bytes = cb::tile_cols_bytes(bv.role_cols, lay.n_slots);
     // [image][tile stage 0][tile stage 1][row_am copy][aset_k copy]
-    const uint64_t small_tabs = (uint64_t)bv.n_asets * lay.n_rows * 8 + (((uint64_t)bv.n_asets + 1) & ~1ull) * 4 + 16 + 2 * kThreads;   // + tile_s[2] + res_s[2][256]
+    const uint64_t small_tabs = n_pk * 8 + (((uint64_t)bv.n_asets + 1) & ~1ull) * 4 + 16 + 2 * kThreads;   // + tile_s[2] + res_s[2][256]
     const uint32_t tiles_smem = ((lay.image_bytes + 127u) & ~127u) + 2 * tile_bytes + (uint32_t)(small_tabs < 65536 ? small_tabs : 65536);
-    auto al16 = [](const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
-    const bool col_tiles = !uc && narrow && stage && !cluster && !ctx->force_no_tiles && tiles_smem <= kMaxTilesSmem && bv.stride % 4 == 0 &&
-                           bv.first % 4 == 0 && al16(bv.hdr0) && al16(bv.hdr1) && al16(bv.roles) && al16(bv.slots);
+    auto al16 = [](const void *ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
+    p.col_tiles = !p.uc && p.lean && p.stage && !p.cluster && !ctx.force_no_tiles && tiles_smem <= kMaxTilesSmem && bv.stride % 4 == 0 &&
+                  bv.first % 4 == 0 && al16(bv.hdr0) && al16(bv.hdr1) && al16(bv.roles) && al16(bv.slots);
     // unique-condition launch: staged (compact image + merged rows in shared memory) when that fits
-    const uint64_t uc_smem64 = uc ? ((t->uc.lay.image_bytes + 127u) & ~127u) + (uint64_t)bv.n_asets * lay.n_rows * 16 : 0;
-    const bool uc_staged = uc && !ctx->force_no_stage && uc_smem64 <= kUcMaxSmem && (!uc_spec_ready || t->spec_uc != nullptr);
-    const uint32_t smem = uc ? (uc_staged ? (uint32_t)uc_smem64 : 0) : col_tiles ? tiles_smem : stage ? lay.image_bytes : 0;
+    p.uc_staged = p.uc && !ctx.force_no_stage && uc_stageable(t.uc, n_pk) && (!uc_spec_ready || t.spec_uc != nullptr);
     // lean launches with a staged table use the kernels specialised for this table when they exist (NVRTC, first use)
-    const bool spec = uc ? uc_spec_ready
-                         : narrow && stage && bv.count < (1ull << 32) && mt->spec_state.load(std::memory_order_acquire) == 1 && t->spec_tiles != nullptr;   // never waits for the compile
-    const void *fn = uc          ? (spec ? (uc_staged ? (const void *)t->spec_uc : (const void *)t->spec_uc_global) : uc_staged ? (const void *)check_uc<true> : (const void *)check_uc<false>)
-                     : spec      ? (col_tiles ? (const void *)t->spec_tiles : (const void *)t->spec_direct)
-                     : col_tiles ? (const void *)check_kernel_tiles
-                     : narrow    ? (stage ? (const void *)check_kernel<true, 1> : (const void *)check_kernel<true, 0>)
-                                 : (const void *)check_kernel<false, 2>;
-    // resident CTAs per SM for this shared-memory footprint: queried once per (table, variant, footprint)
-    const int variant = uc ? (spec ? (uc_staged ? 9 : 10) : uc_staged ? 7 : 8) : spec ? (col_tiles ? 5 : 6) : col_tiles ? 4 : narrow ? (stage ? 1 : 2) : (stage ? 0 : 3);
-    int occ = mt->occ_smem[variant].load(std::memory_order_relaxed) == smem + 1 ? mt->occ[variant].load(std::memory_order_relaxed) : 0;
-    if (occ == 0) {
-        if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxStageBytes) != cudaSuccess ||
-            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, kThreads, smem) != cudaSuccess) {
-            if (!spec) return fail(CGPU_ERR_CUDA, "kernel attribute / occupancy query failed: %s", cudaGetErrorString(cudaGetLastError()));
-            cudaGetLastError();
-            occ = CB_MIN_BLOCKS;   // run-time loaded kernel on a runtime that cannot query it: the launch-bounds minimum
-        }
-        if (occ < 1) occ = 1;
-        mt->occ[variant].store(occ, std::memory_order_relaxed);
-        mt->occ_smem[variant].store(smem + 1, std::memory_order_relaxed);
+    p.spec = p.uc ? uc_spec_ready : p.lean && p.stage && bv.count < (1ull << 32) && spec_ready && t.spec_tiles != nullptr;
+    p.kernel = p.uc        ? (p.spec ? (p.uc_staged ? Kernel::SpecUc : Kernel::SpecUcGlobal) : p.uc_staged ? Kernel::Uc : Kernel::UcGlobal)
+             : p.spec      ? (p.col_tiles ? Kernel::SpecTiles : Kernel::SpecDirect)
+             : p.col_tiles ? Kernel::LeanTiles
+             : p.lean      ? (p.stage ? Kernel::Lean : Kernel::LeanGlobal)
+                           : (p.stage ? Kernel::General : Kernel::GeneralGlobal);
+    p.smem = p.uc ? (p.uc_staged ? (uint32_t)uc_smem_bytes(t.uc, n_pk) : 0) : p.col_tiles ? tiles_smem : p.stage ? lay.image_bytes : 0;
+    p.last_arg = p.col_tiles ? lay.n_slots : p.stage ? 1u : 0u;
+    p.serialise = p.spec && !p.uc && !ctx.profiling;
+    p.strpred = p.uc && p.spec && t.spec_n_strpred;
+    // on a global image the rows are merged with the batch's action-set masks once, up front
+    p.merge_rows = p.uc && !p.uc_staged && n_pk <= (1u << 19);
+    return p;
+}
+
+const void *kernel_fn(const cgpu_table &t, Kernel k) {
+    switch (k) {
+    case Kernel::General:
+    case Kernel::GeneralGlobal: return (const void *)check_kernel<false, 2>;
+    case Kernel::Lean: return (const void *)check_kernel<true, 1>;
+    case Kernel::LeanGlobal: return (const void *)check_kernel<true, 0>;
+    case Kernel::LeanTiles: return (const void *)check_kernel_tiles;
+    case Kernel::Uc: return (const void *)check_uc<true>;
+    case Kernel::UcGlobal: return (const void *)check_uc<false>;
+    case Kernel::SpecTiles: return (const void *)t.spec_tiles;
+    case Kernel::SpecDirect: return (const void *)t.spec_direct;
+    case Kernel::SpecUc: return (const void *)t.spec_uc;
+    case Kernel::SpecUcGlobal: return (const void *)t.spec_uc_global;
     }
-    uint64_t max_ctas = (uint64_t)ctx->sm_count * (uint64_t)occ;
+    return nullptr;
+}
+
+// Resident CTAs per SM of kernel k with `smem` bytes of dynamic shared memory, queried once per (table, kernel, footprint);
+// also lifts the kernel's dynamic shared-memory limit to kMaxStageBytes.  A CGPU_ERR_* code (< 0) when the query fails.
+int resident_ctas(const cgpu_table &t, Kernel k, uint32_t smem) {
+    std::atomic<uint64_t> &entry = t.occ[(int)k];
+    const uint64_t e = entry.load(std::memory_order_relaxed);
+    if ((uint32_t)e != 0 && (uint32_t)(e >> 32) == smem) return (int)(uint32_t)e;
+    const void *fn = kernel_fn(t, k);
+    int occ = 0;
+    if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxStageBytes) != cudaSuccess ||
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, kThreads, smem) != cudaSuccess) {
+        if (k < Kernel::SpecTiles) return fail(CGPU_ERR_CUDA, "kernel attribute / occupancy query failed: %s", cudaGetErrorString(cudaGetLastError()));
+        cudaGetLastError();
+        occ = CB_MIN_BLOCKS;   // run-time loaded kernel on a runtime that cannot query it: the launch-bounds minimum
+    }
+    if (occ < 1) occ = 1;
+    entry.store((uint64_t)smem << 32 | (uint32_t)occ, std::memory_order_relaxed);
+    return occ;
+}
+
+// Launches fn programmatically serialised behind the kernel before it on `stream`: its CTAs may start while that kernel's
+// last ones still run, and wait for it (griddepcontrol.wait) before they read what it wrote.
+cudaError_t launch_serialised(const void *fn, uint32_t grid, uint32_t block, uint32_t smem, cudaStream_t stream, void **args) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(block); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+    cudaLaunchAttribute pdl[1];
+    pdl[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    pdl[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = pdl; cfg.numAttrs = 1;
+    return cudaLaunchKernelExC(&cfg, fn, args);
+}
+
+// Issues the launches of `plan` (plan_launch for this table and batch) on `stream`.
+int launch_check(cgpu_ctx *ctx, const cgpu_table *t, const LaunchPlan &plan, const cb::BatchView &bv, uint8_t *d_bitmap, uint8_t *d_effects,
+                 uint32_t *d_status, cudaStream_t stream) {
+    const cb::TableLayout &lay = t->desc.lay;
+    const uint64_t tiles = (bv.count + kThreads - 1) / kThreads;
+    const int occ = resident_ctas(*t, plan.kernel, plan.smem);
+    if (occ < 0) return occ;
+    const uint64_t max_ctas = (uint64_t)ctx->sm_count * (uint64_t)occ;
     uint32_t grid = (uint32_t)(tiles < max_ctas ? tiles : max_ctas);
     if (grid == 0) grid = 1;
-    TableDesc td = uc ? t->uc_desc : t->desc;
+    TableDesc td = plan.uc ? t->uc_desc : t->desc;
     cb::BatchView bvv = bv;
     bvv.perm = nullptr;
     // few slot columns: every tile prefetches all of them one tile ahead (all loads of the tile then hit L1);
     // otherwise each policy block prefetches the slots its own conditions read
     bvv.prefetch_slots = lay.n_slots <= 8 ? lay.n_slots : 0;
     uint32_t *perm = nullptr;
-    if (cluster) {
+    if (plan.cluster) {
         int rc = launch_cluster(ctx, t, bv, &perm, stream);
         if (rc != CGPU_OK) return rc;
         bvv.perm = perm;
     }
-    uint32_t last_arg = col_tiles ? lay.n_slots : (stage ? 1u : 0u);   // check_kernel: stage_rt; check_kernel_tiles: n_slots
-    const bool lists = narrow;       // requests a lean kernel leaves to the general kernel go to a list drained right behind it
+    uint32_t last_arg = plan.last_arg;
     uint32_t *defer = nullptr;
-    if (lists) {
+    if (plan.lean) {   // requests a lean kernel leaves to the general kernel go to a list drained right behind it
         uint32_t *cell = nullptr, *strpred = nullptr;
-        const bool want_sp = uc && spec && t->spec_n_strpred;
-        const uint32_t n_str = lay.nT + bv.n_bstr;
-        // unique-condition launch on a global image: merge the rows with the batch's action-set masks once, up front
-        const uint64_t n_pk = (uint64_t)bv.n_asets * lay.n_rows;
-        const bool want_pk = uc && !uc_staged && n_pk <= (1u << 19);
         cb::U4 *pk = nullptr;
-        int rc = acquire_defer(ctx, stream, bv.count, &defer, &cell, (size_t)n_str + 1, want_sp ? &strpred : nullptr, (size_t)n_pk, want_pk ? &pk : nullptr);
+        const uint32_t n_str = lay.nT + bv.n_bstr;
+        const uint64_t n_pk = (uint64_t)bv.n_asets * lay.n_rows;
+        int rc = acquire_defer(ctx, stream, bv.count, &defer, &cell, plan.strpred ? (size_t)n_str + 1 : 0, &strpred, plan.merge_rows ? (size_t)n_pk : 0, &pk);
         if (rc != CGPU_OK) return rc;
-        if (want_pk) {
+        if (plan.merge_rows) {
             uc_merge_rows<<<(unsigned)((n_pk + kThreads - 1) / kThreads), kThreads, 0, stream>>>(t->uc_desc, bvv, pk, (uint32_t)n_pk);
             CUDA_TRY(cudaGetLastError());
             ctx->launches.fetch_add(1, std::memory_order_relaxed);
             bvv.uc_rows_pk = pk;
         }
         bvv.defer_count = cell;
-        bvv.tile_counter = col_tiles ? cell + 2 : nullptr;
+        bvv.tile_counter = plan.col_tiles ? cell + 2 : nullptr;
         bvv.defer_list = defer;
-        if (want_sp && n_str) {
+        if (plan.strpred && n_str) {
             // string predicates against constants: evaluated once per distinct string of the dictionary, not once per request
             TableDesc ptd = t->uc_desc;
             uint32_t n_arg = n_str;
@@ -983,6 +1055,7 @@ int launch_check(cgpu_ctx *ctx, const cgpu_table *t, const cb::BatchView &bv, ui
         }
         bvv.strpred = strpred;
     }
+    const void *fn = kernel_fn(*t, plan.kernel);
     void *args[] = {&td, &bvv, &d_bitmap, &d_effects, &d_status, &last_arg};
     if (ctx->profiling) {
         if (ctx->prof_pending && cudaEventSynchronize(ctx->ev1) == cudaSuccess) {
@@ -992,63 +1065,41 @@ int launch_check(cgpu_ctx *ctx, const cgpu_table *t, const cb::BatchView &bv, ui
         }
         CUDA_TRY(cudaEventRecord(ctx->ev0, stream));
     }
-    if (spec && !uc && !ctx->profiling) {
-        // programmatically serialised behind the previous launch's drain kernel (which releases its dependents at once):
-        // this kernel's CTAs start as the previous specialised kernel's last tiles retire -- back-to-back launches on one
-        // stream overlap at their tails.  It reads nothing the previous launch writes.
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-        cudaLaunchAttribute pdl[1];
-        pdl[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        pdl[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = pdl; cfg.numAttrs = 1;
-        CUDA_TRY(cudaLaunchKernelExC(&cfg, fn, args));
+    if (plan.serialise) {
+        // behind the previous launch's drain kernel (which releases its dependents at once): this kernel's CTAs start as the
+        // previous specialised kernel's last tiles retire -- back-to-back launches on one stream overlap at their tails.
+        // It reads nothing the previous launch writes.
+        CUDA_TRY(launch_serialised(fn, grid, kThreads, plan.smem, stream, args));
     } else {
-        CUDA_TRY(cudaLaunchKernel(fn, dim3(grid), dim3(kThreads), args, smem, stream));
+        CUDA_TRY(cudaLaunchKernel(fn, dim3(grid), dim3(kThreads), args, plan.smem, stream));
     }
     CUDA_TRY(cudaGetLastError());
     if (ctx->profiling) { CUDA_TRY(cudaEventRecord(ctx->ev1, stream)); ctx->prof_pending = true; }
-    if (lists) {
-        // drain the deferral list with the general body (usually empty: the kernel then exits at once)
+    if (plan.lean) {
+        // drain the deferral list with the general body (usually empty: the kernel then exits at once); it also does the
+        // fused-gather signalling (BatchView::sig_*)
         cb::BatchView dv = bv;
         dv.perm = defer;
         dv.count_dev = bvv.defer_count;
         dv.prefetch_slots = 0;
-        const void *gfn = (const void *)check_kernel<false, 2>;
-        const uint32_t gsmem = stage ? lay.image_bytes : 0;
-        int gocc = mt->occ[0].load(std::memory_order_relaxed);
-        if (gocc == 0 || mt->occ_smem[0].load(std::memory_order_relaxed) != gsmem + 1) {
-            CUDA_TRY(cudaFuncSetAttribute(gfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxStageBytes));
-            CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&gocc, gfn, kThreads, gsmem));
-            if (gocc < 1) gocc = 1;
-            mt->occ[0].store(gocc, std::memory_order_relaxed);
-            mt->occ_smem[0].store(gsmem + 1, std::memory_order_relaxed);
-        }
+        const Kernel gk = plan.stage ? Kernel::General : Kernel::GeneralGlobal;
+        const uint32_t gsmem = plan.stage ? lay.image_bytes : 0;
+        const int gocc = resident_ctas(*t, gk, gsmem);   // (for the shared-memory limit it sets: the grid does not depend on it)
+        if (gocc < 0) return gocc;
         // one CTA per SM: the list is normally empty (every CTA then exits at once), and grid-stride loops otherwise
-        uint64_t gmax = (uint64_t)ctx->sm_count;
-        uint32_t ggrid = (uint32_t)(tiles < gmax ? tiles : gmax);
-        uint32_t stage_arg = stage ? 1u : 0u;
-        uint8_t *gb = d_bitmap, *ge = d_effects;
+        const uint64_t gmax = (uint64_t)ctx->sm_count;
+        const uint32_t ggrid = (uint32_t)(tiles < gmax ? tiles : gmax);
+        uint32_t stage_arg = plan.stage ? 1u : 0u;
         TableDesc gtd = t->desc;
-        void *gargs[] = {&gtd, &dv, &gb, &ge, &d_status, &stage_arg};
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(ggrid ? ggrid : 1); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = gsmem; cfg.stream = stream;
-        cudaLaunchAttribute pdl[1];
-        pdl[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        pdl[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = pdl; cfg.numAttrs = 1;
-        CUDA_TRY(cudaLaunchKernelExC(&cfg, gfn, gargs));
+        void *gargs[] = {&gtd, &dv, &d_bitmap, &d_effects, &d_status, &stage_arg};
+        CUDA_TRY(launch_serialised(kernel_fn(*t, gk), ggrid ? ggrid : 1, kThreads, gsmem, stream, gargs));
         CUDA_TRY(cudaGetLastError());
         ctx->launches.fetch_add(1, std::memory_order_relaxed);
-        if (drained) *drained = true;   // the drain kernel also did the fused-gather signalling (BatchView::sig_*)
     }
     if (perm) CUDA_TRY(cudaFreeAsync(perm, stream));
     ctx->launches.fetch_add(1, std::memory_order_relaxed);
-    ctx->last_grid = grid; ctx->last_block = kThreads; ctx->last_smem = smem; ctx->last_fast = narrow ? 1 : 0;
-    ctx->last_clustered = cluster ? 1 : 0;
-    ctx->last_col_tiles = col_tiles ? 1 : 0;
-    ctx->last_spec = spec ? 1 : 0;
-    ctx->last_uc = uc ? 1 : 0;
+    ctx->last_plan = plan;
+    ctx->last_grid = grid;
     return CGPU_OK;
 }
 
@@ -1140,9 +1191,7 @@ void cgpu_shutdown(cgpu_ctx *ctx) {
     }
     if (ctx->d_status) cudaFree(ctx->d_status);
     for (auto &kv : ctx->defer_lanes) {
-        for (auto p : kv.second.lists) if (p) cudaFree(p);
-        for (auto p : kv.second.strpred) if (p) cudaFree(p);
-        for (auto p : kv.second.pk) if (p) cudaFree(p);
+        for (auto &b : kv.second.q) { cudaFree(b.list.ptr); cudaFree(b.strpred.ptr); cudaFree(b.pk.ptr); }
         if (kv.second.cells) cudaFree(kv.second.cells);
     }
     if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
@@ -1282,14 +1331,15 @@ int cgpu_deferred_count(cgpu_ctx *ctx, uint64_t *total) {
 int cgpu_last_kernel_config(const cgpu_ctx *ctx, uint32_t *grid, uint32_t *block, uint32_t *smem_bytes) {
     if (!ctx) return fail(CGPU_ERR_INVALID, "null ctx");
     if (grid) *grid = ctx->last_grid;
-    if (block) *block = ctx->last_block;
-    if (smem_bytes) *smem_bytes = ctx->last_smem | (ctx->last_fast << 31);   // bit 31: lean kernel body was used
+    if (block) *block = ctx->last_grid ? kThreads : 0;   // 0 before the first launch
+    if (smem_bytes) *smem_bytes = ctx->last_plan.smem | (uint32_t)ctx->last_plan.lean << 31;   // bit 31: lean kernel body was used
     return CGPU_OK;
 }
 
 int cgpu_last_cluster_config(const cgpu_ctx *ctx, uint32_t *clustered, uint32_t *window, uint32_t *buckets) {
     if (!ctx) return fail(CGPU_ERR_INVALID, "null ctx");
-    if (clustered) *clustered = ctx->last_clustered | (ctx->last_col_tiles << 1) | (ctx->last_spec << 2) | (ctx->last_uc << 3);   // bit 1: TMA column tiles; bit 2: table-specialised kernel
+    const LaunchPlan &p = ctx->last_plan;
+    if (clustered) *clustered = (uint32_t)p.cluster | (uint32_t)p.col_tiles << 1 | (uint32_t)p.spec << 2 | (uint32_t)p.uc << 3;   // include/cerbos_b200.h
     if (window) *window = ctx->last_window;
     if (buckets) *buckets = ctx->last_buckets;
     return CGPU_OK;
@@ -1321,7 +1371,7 @@ int cgpu_check_device(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *dev_
     if (rc != CGPU_OK) return rc;
     CUDA_TRY(cudaSetDevice(ctx->device));
     cudaStream_t s = static_cast<cudaStream_t>(cuda_stream);   // NULL = the legacy default stream
-    return launch_check(ctx, t, bv, static_cast<uint8_t *>(dev_bitmap_out), nullptr, ctx->d_status, s);
+    return launch_check(ctx, t, plan_launch(*ctx, *t, bv), bv, static_cast<uint8_t *>(dev_bitmap_out), nullptr, ctx->d_status, s);
 }
 
 int cgpu_peer_alloc(cgpu_ctx *ctx, size_t bytes, void **dev_ptr, void *ipc_handle_out) {
@@ -1416,7 +1466,7 @@ int cgpu_check_device_gather(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batc
             CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&use->stage), slice_used));
             use->stage_bytes = slice_used;
         }
-        rc = launch_check(ctx, t, bv, use->stage, nullptr, ctx->d_status, s);
+        rc = launch_check(ctx, t, plan_launch(*ctx, *t, bv), bv, use->stage, nullptr, ctx->d_status, s);
         if (rc != CGPU_OK) return rc;
         cudaEvent_t &ev = ctx->copy_ev[ctx->copy_seq++ & 15];
         if (!ev) CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
@@ -1443,18 +1493,12 @@ int cgpu_check_device_gather(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batc
     for (uint32_t r = 0; r < g->n_ranks; r++) bv.sig_flags[r] = g->flags[r];
     bv.sig_rank = g->my_rank; bv.sig_step = g->step;
     bv.wait_flags = sp.wait_flags; bv.wait_step = g->wait_step;
-    bool drained = false;
-    rc = launch_check(ctx, t, bv, bv.outs[g->my_rank], nullptr, ctx->d_status, s, &drained);
+    const LaunchPlan plan = plan_launch(*ctx, *t, bv);
+    rc = launch_check(ctx, t, plan, bv, bv.outs[g->my_rank], nullptr, ctx->d_status, s);
     if (rc != CGPU_OK) return rc;
-    if (!drained) {   // generic kernels: a one-warp kernel behind them publishes the step (and does the lagged wait)
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(1); cfg.blockDim = dim3(32); cfg.stream = s;
-        cudaLaunchAttribute pdl[1];
-        pdl[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        pdl[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = pdl; cfg.numAttrs = 1;
+    if (!plan.lean) {   // no drain kernel to do the signalling: a one-warp kernel behind the check publishes the step (and does the lagged wait)
         void *args[] = {&sp};
-        CUDA_TRY(cudaLaunchKernelExC(&cfg, (const void *)gather_signal, args));
+        CUDA_TRY(launch_serialised((const void *)gather_signal, 1, 32, 0, s, args));
         ctx->launches.fetch_add(1, std::memory_order_relaxed);
     }
     return CGPU_OK;
@@ -1912,7 +1956,7 @@ static int check_range(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *bat
         cb::BatchView cv = bv;
         cv.first = c0; cv.count = cnt;
         // the kernel writes effect bytes directly (1 ALLOW / 2 DENY / 0 padding): no host post-pass
-        rc = launch_check(ctx, t, cv, nullptr, d_effects, slot->d_status, slot->stream);
+        rc = launch_check(ctx, t, plan_launch(*ctx, *t, cv), cv, nullptr, d_effects, slot->d_status, slot->stream);
         if (rc != CGPU_OK) return rc;
         CUDA_TRY(cudaEventRecord(slot->ev[2 * k + 1], slot->stream));
         CUDA_TRY(cudaStreamWaitEvent(slot->d2h, slot->ev[2 * k + 1], 0));

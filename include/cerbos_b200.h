@@ -243,7 +243,8 @@ int cgpu_last_kernel_config(const cgpu_ctx *ctx, uint32_t *grid, uint32_t *block
 /* Whether the last launch evaluated in clustered order (requests grouped by policy block inside L2-sized windows by
  * three small kernels ahead of the check kernel; env CERBOS_B200_CLUSTER=0/1 overrides the batch-size rule).
  * *clustered bit 0: clustered order; bit 1: the request columns were staged tile by tile through TMA; bit 2: the
- * kernel was the one compiled for this table at run time (NVRTC; env CERBOS_B200_NO_JIT=1 disables). */
+ * kernel was the one compiled for this table at run time (NVRTC; env CERBOS_B200_NO_JIT=1 disables); bit 3: a
+ * unique-condition kernel (env CERBOS_B200_UC=0/1 overrides the block-shape rule). */
 int cgpu_last_cluster_config(const cgpu_ctx *ctx, uint32_t *clustered, uint32_t *window, uint32_t *buckets);
 /* Returns and resets the CUDA-event time (ms) spent in the check kernel itself over the launches since the last
  * call, then switches the per-launch events on or off. Measurement aid for bench.py; off by default. */

@@ -223,7 +223,9 @@ inline std::string atom_source(const std::vector<Ins> &P, uint32_t lo, uint32_t 
             if (d < 2) bad = true;
             nd = d - 1; break;
         case CB_OP_HIER_CA: nd = d - (I.ia == 0 ? 1 : 2); if (nd < 1) bad = true; break;
-        case CB_OP_FN: if (I.ib < 1 || I.ib > 4 || d < (int)I.ib) bad = true; nd = d - ((int)I.ib - 1); break;
+        case CB_OP_FN:   // (format takes its clause record and the list literal's elements: up to a full stack)
+            if (I.ib < 1 || I.ib > (I.ia == CB_FN_FORMAT ? (uint32_t)CB_MAX_STACK : 4u) || d < (int)I.ib) bad = true;
+            nd = d - ((int)I.ib - 1); break;
         case CB_OP_JF_KEEP: case CB_OP_JT_KEEP: if (d < 1) bad = true; set(rel(I.ic), d, l); target[rel(I.ic)] = true; break;
         case CB_OP_JMP: set(rel(I.ic), d, l); target[rel(I.ic)] = true; falls = false; break;
         case CB_OP_TERN:

@@ -56,7 +56,9 @@ __global__ void __launch_bounds__(kThreads, CB_MIN_BLOCKS) check_kernel_tiles(co
 }
 
 // decision-metadata kernel (cgpu_check_meta): one thread per request, the reference's own loop order (cb::eval_request_meta)
-__global__ void __launch_bounds__(kThreads) check_meta_kernel(const __grid_constant__ TableDesc td, const __grid_constant__ cb::BatchView bv, uint8_t *effects,
+// Two resident CTAs (up to 128 registers), stated: left to ptxas, this kernel's register budget moves with the size of the
+// interpreter's call graph, and it fell to 32 registers with heavy spills once the format printers joined it
+__global__ void __launch_bounds__(kThreads, 2) check_meta_kernel(const __grid_constant__ TableDesc td, const __grid_constant__ cb::BatchView bv, uint8_t *effects,
                                                              uint32_t *action_meta, cb_request_meta *req_meta, uint32_t *status) {
     for (uint64_t i = (uint64_t)blockIdx.x * kThreads + threadIdx.x; i < bv.count; i += (uint64_t)gridDim.x * kThreads)
         cb::eval_request_meta(td.base, &td.lay, &bv, bv.first + i, effects, action_meta, req_meta, status);

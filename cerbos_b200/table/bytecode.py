@@ -17,7 +17,8 @@ What is lowered
     expression is equally an error; ``has(V.x)`` -> NOERR);
   * operators, ``in``, index/select, size, startsWith/endsWith/contains,
     hasIntersection/isSubset, all/exists/exists_one (1- and 2-variable),
-    ternary, numeric/timestamp/duration conversions, now()/timeSince().
+    ternary, numeric/timestamp/duration conversions, now()/timeSince(), format() with a constant format string and
+    strings.quote (ext.Strings).
 
 Anything else raises :class:`Unsupported` -- table build fails loudly; there is no
 silent per-request divergence and no CPU fallback (SURVEY.md 8(b)).
@@ -825,6 +826,8 @@ class ProgramCompiler:
                 self.expr(a)
             self.emit("FN", a=L.FNS[self._MATH[fn][0]], b=len(args), delta=1 - len(args))
             return
+        if fn == "format" and n.target is not None and len(n.args) == 1:
+            return self._format(n.target, n.args[0])
         if fn in self._FN and len(args) in self._FN[fn][1]:
             # string / list producing functions (ext.Strings, ext.Lists, Cerbos except / intersect): results live in the
             # device's per-thread scratch arena
@@ -845,7 +848,43 @@ class ProgramCompiler:
            "indexOf": ("INDEXOF", (2, 3)), "lastIndexOf": ("LASTINDEXOF", (2, 3)), "substring": ("SUBSTRING", (2, 3)),
            "replace": ("REPLACE", (3, 4)), "split": ("SPLIT", (2, 3)), "join": ("JOIN", (1, 2)), "reverse": ("REVERSE", (1,)),
            "except": ("EXCEPT", (2,)), "intersect": ("INTERSECT", (2,)), "sort": ("SORT", (1,)), "slice": ("SLICE", (3,)),
-           "flatten": ("FLATTEN", (1, 2)), "distinct": ("DISTINCT", (1,)), "lists.range": ("RANGE", (1,))}
+           "flatten": ("FLATTEN", (1, 2)), "distinct": ("DISTINCT", (1,)), "lists.range": ("RANGE", (1,)),
+           "strings.quote": ("QUOTE", (1,))}
+
+    def _format(self, target: Node, arg: Node):
+        """fmt.format(args) (ext.Strings) with a constant fmt: its clauses are parsed here, once, into a THEAP record (layout
+        FORMAT).  A list-literal `args` of up to FORMAT_MAX_STACK_ARGS elements is compiled element by element onto the stack,
+        so no list is built at run time and the condition stays within the leaf-program translator; a longer literal (or any
+        other list value) is one operand, the list."""
+        fmt = None
+        if isinstance(target, Const) and isinstance(target.value, str):
+            fmt = target.value
+        else:
+            s = self._simple(target)
+            if s is not None and s[0] == "const" and isinstance(s[1][0], str):
+                fmt = s[1][0]
+        if fmt is None:
+            raise Unsupported("format() with a format string that is not a constant")
+        items = parse_format(fmt)
+        if items is None:
+            # a clause that cannot be parsed is an error whatever the arguments are (every clause is reached)
+            self.push_const(ConstVal(T["ERR"], 0))
+            return
+        words = [len(items)]
+        for it in items:
+            if it[0] == "lit":
+                words.append(self.ctx.strings.intern(it[1]) << 32)
+            else:
+                prec = L.FMT_PREC_DEFAULT if it[2] is None else min(it[2], L.FMT_PREC_DEFAULT - 1)
+                words.append(ord(it[1]) | (prec << 16))
+        rec = self.ctx._heap_put(words)
+        direct = isinstance(arg, ListLit) and len(arg.elems) <= FORMAT_MAX_STACK_ARGS
+        mode = L.FORMAT_ARGS_STACK if direct else L.FORMAT_ARGS_LIST
+        self.push_const(ConstVal(T["INT"], rec | (mode << 32)))
+        args = arg.elems if direct else [arg]
+        for e in args:
+            self.expr(e)
+        self.emit("FN", a=L.FNS["FORMAT"], b=1 + len(args), delta=-len(args))
 
     # ---- SPIFFE (conditions/types/spiffe.go): ids and trust domains are strings of a validated shape (tags SPIFFE_ID /
     # SPIFFE_TD); a matcher is never a run-time value -- spiffeMatchX(arg).matchesID(x) compiles to one fused function
@@ -1022,6 +1061,53 @@ class ProgramCompiler:
     def finish(self):
         self.emit("RET")
         return self.code
+
+
+_FMT_VERBS = "sdfebxXo"
+# list-literal elements FORMAT takes from the operand stack: with the clause record and the enclosing expression's operands
+# they must fit the device's evaluation stack (layout.MAX_STACK = 16)
+FORMAT_MAX_STACK_ARGS = L.MAX_STACK - 4
+
+
+def parse_format(fmt: str):
+    """Clauses of a format string as cel-go's ext.Strings reads them (restated by oracle #1, celeval._str_format):
+    [("lit", text) | ("verb", verb, precision or None)], or None when a clause is malformed -- a lone `%` at the end, a
+    precision with no verb after it, or a verb outside %s %d %f %e %b %x %X %o -- which makes every call an error."""
+    items, lit = [], []
+    i, n = 0, len(fmt)
+    while i < n:
+        ch = fmt[i]
+        if ch != "%":
+            lit.append(ch)
+            i += 1
+            continue
+        i += 1
+        if i >= n:
+            return None
+        if fmt[i] == "%":
+            lit.append("%")
+            i += 1
+            continue
+        prec = None
+        if fmt[i] == ".":
+            j = i + 1
+            while j < n and fmt[j].isdigit():
+                j += 1
+            digits = fmt[i + 1:j]
+            if not digits.isascii():
+                raise Unsupported("format() clause with a precision in non-ASCII digits")
+            prec = int(digits or "0")
+            i = j
+        if i >= n or fmt[i] not in _FMT_VERBS:
+            return None
+        if lit:
+            items.append(("lit", "".join(lit)))
+            lit = []
+        items.append(("verb", fmt[i], prec))
+        i += 1
+    if lit:
+        items.append(("lit", "".join(lit)))
+    return items
 
 
 def _substitute(node, name, repl, repl_free):

@@ -156,6 +156,14 @@ OPS = {name: i for i, name in enumerate([
     "MATCHES",          # TOS string -> BOOL: RE2 search with the byte-level DFA at theap[c] (cel/regex_dfa.py)
     "RUNTIME_EDR",      # push runtime.effectiveDerivedRoles: the derived roles in force for the policy being evaluated (list of strings)
 ])}
+# FN FORMAT: fmt.format(args) with a constant fmt (ext.Strings).  Its first argument is an INT constant: the THEAP offset of the
+# parsed clause record | mode << 32.  FORMAT_ARGS_STACK: the remaining arguments are the list literal's elements;
+# FORMAT_ARGS_LIST: the one remaining argument is the list.  The clause record is [n items, then one word per item]; an item is
+# a literal run (verb byte 0, table string id in bits 32..63) or a clause (verb byte 's' 'd' 'f' 'e' 'b' 'x' 'X' 'o', precision
+# in bits 16..31, FMT_PREC_DEFAULT = none given)
+FORMAT_ARGS_STACK = 0
+FORMAT_ARGS_LIST = 1
+FMT_PREC_DEFAULT = 0xFFFF
 # FN ids: string functions first (cel-go ext.Strings), list functions from EXCEPT on (ext.Lists, Cerbos except / intersect)
 FNS = {name: i for i, name in enumerate([
     "LOWER", "UPPER", "TRIM", "STR_REVERSE", "CHARAT", "INDEXOF", "LASTINDEXOF", "SUBSTRING", "REPLACE", "SPLIT", "JOIN",
@@ -173,6 +181,8 @@ FNS = {name: i for i, name in enumerate([
     "TO_STRING",        # string(x): strings, ints, uints, bools, valid UTF-8 bytes, integral doubles below 2^53 (the rest is flagged)
     "TYPE_OF",          # type(x) -> a TYPE value (payload: TYPE_CODES); type names are TYPE constants, compared by payload
     "TO_BOOL",          # bool(x): a bool, or a string strconv.ParseBool reads ("1" "t" "T" "TRUE" "true" "True" / "0" "f" "F" "FALSE" "false" "False")
+    "QUOTE",            # strings.quote(s): s in double quotes, \a \b \f \n \r \t \v \\ and \" escaped
+    "FORMAT",           # [record, args...]: fmt.format(args) by a parsed clause record (FORMAT_ARGS_* below)
 ])}
 # payload of a TYPE value (type(x), the identifiers int / string / ... in an expression)
 TYPE_CODES = {"bool": 1, "int": 2, "uint": 3, "double": 4, "string": 5, "bytes": 6, "list": 7, "map": 8, "null_type": 9,
@@ -308,6 +318,9 @@ def c_header() -> str:
     d("CB_MAX_ROLE_COLS", MAX_ROLE_COLS)
     d("CB_MAX_CLASS_PATS", MAX_CLASS_PATS)
     d("CB_BATCH_FLAG_LENIENT", BATCH_FLAG_LENIENT)
+    d("CB_FORMAT_ARGS_STACK", FORMAT_ARGS_STACK)
+    d("CB_FORMAT_ARGS_LIST", FORMAT_ARGS_LIST)
+    d("CB_FMT_PREC_DEFAULT", FMT_PREC_DEFAULT, True)
     for k, v in META_SRC.items():
         d(f"CB_META_SRC_{k}", v)
     out.append("")

@@ -1040,8 +1040,7 @@ CB_HD_NOINLINE Val conv_uint(Ctx &c, const Val &v) {
         uint32_t n;
         str_get(c, v.u, p, n);
         uint32_t i = 0;
-        if (n && ldg(p) == '+') i = 1;
-        if (i == n) return mk_err();
+        if (n == 0) return mk_err();      // strconv.ParseUint(s, 10, 64): digits only, "A sign prefix is not permitted"
         uint64_t acc = 0;
         for (; i < n; i++) {
             uint8_t ch = ldg(p + i);
@@ -1829,7 +1828,9 @@ CB_HD_NOINLINE void shortest_digits(uint64_t bits, uint64_t *f, int *e) {
     const uint64_t g1 = schubfach_g(gi), g0 = schubfach_g(gi + 1);
     const uint64_t vb = schubfach_rop(g1, g0, cb << h), vbl = schubfach_rop(g1, g0, cbl << h), vbr = schubfach_rop(g1, g0, cbr << h);
     const uint64_t s = vb >> 2;
-    if (s >= 100) {
+    // one digit fewer, when that still rounds to the double.  The paper tries it from s >= 100 only (Java prints at least two
+    // digits); Go prints the shortest, so the subnormals with s in 10..99 (c = 3..20) try it too: 8e-323, not 7.9e-323.
+    if (s >= 10) {
         const uint64_t sp10 = s / 10 * 10, tp10 = sp10 + 10;
         const bool upin = vbl + out <= sp10 << 2, wpin = (tp10 << 2) + out <= vbr;
         if (upin != wpin) { *f = upin ? sp10 : tp10; *e = k; return; }

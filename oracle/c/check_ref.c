@@ -756,8 +756,8 @@ static val_t conv_uint(ectx_t *c, val_t v) {
     case CB_T_DOUBLE: { double d = as_double(v); if (d != d || d < 0 || d >= 18446744073709551616.0) return mk_err(); return mk(CB_T_UINT, (uint64_t)d); }
     case CB_T_STRING: {
         const uint8_t *p; uint32_t n; str_get(c, v.u, &p, &n);
-        uint32_t i = 0; if (n && p[0] == '+') i = 1;
-        if (i == n) return mk_err();
+        uint32_t i = 0;
+        if (n == 0) return mk_err();   /* strconv.ParseUint(s, 10, 64): digits only, "A sign prefix is not permitted" */
         uint64_t acc = 0;
         for (; i < n; i++) {
             if (p[i] < '0' || p[i] > '9') return mk_err();

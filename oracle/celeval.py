@@ -816,7 +816,7 @@ def conv_uint(v):
             raise CelError("unsigned integer overflow")
         return _chk_uint(int(v))
     if isinstance(v, str):
-        if not re.fullmatch(r"\+?[0-9]+", v):
+        if not re.fullmatch(r"[0-9]+", v):     # strconv.ParseUint(s, 10, 64): "A sign prefix is not permitted"
             raise CelError(f"cannot convert {v!r} to uint")
         return _chk_uint(int(v))
     raise no_overload("uint", v)
@@ -2127,6 +2127,13 @@ def _round_half_away(d):
     return math.copysign(f + 1.0 if abs(d) - f >= 0.5 else f, d)
 
 
+def _keep_zero_sign(fn, d):
+    """Go's math.Ceil / Floor / Trunc: +-Inf and NaN unchanged, a zero result keeps the argument's sign (Ceil(-0.5) = -0)"""
+    if math.isnan(d) or math.isinf(d):
+        return d
+    return math.copysign(0.0, d) if fn(d) == 0 else float(fn(d))
+
+
 def _abs_int(v):
     if v == INT64_MIN:
         raise CelError("integer overflow")
@@ -2347,10 +2354,10 @@ _FUNCS = {
     "lists.range": _f_lists_range, "distinct": _f_distinct, "flatten": _f_flatten, "slice": _f_slice,
     "sort": _f_sort, "first": _f_first, "last": _f_last,
     "math.greatest": _minmax("max", True), "math.least": _minmax("min", False),
-    "math.ceil": _math1("math.ceil", fd=lambda d: float(math.ceil(d)) if math.isfinite(d) else d),
-    "math.floor": _math1("math.floor", fd=lambda d: float(math.floor(d)) if math.isfinite(d) else d),
+    "math.ceil": _math1("math.ceil", fd=lambda d: _keep_zero_sign(math.ceil, d)),
+    "math.floor": _math1("math.floor", fd=lambda d: _keep_zero_sign(math.floor, d)),
     "math.round": _math1("math.round", fd=_round_half_away),
-    "math.trunc": _math1("math.trunc", fd=lambda d: float(math.trunc(d)) if math.isfinite(d) else d),
+    "math.trunc": _math1("math.trunc", fd=lambda d: _keep_zero_sign(math.trunc, d)),
     "math.abs": _math1("math.abs", fi=_abs_int, fu=lambda u: u, fd=abs),
     "math.sign": _math1("math.sign", fi=lambda i: (i > 0) - (i < 0), fu=lambda u: UInt(1 if u > 0 else 0), fd=_sign_d),
     "math.isNaN": _math1("math.isNaN", fd=math.isnan), "math.isInf": _math1("math.isInf", fd=math.isinf),

@@ -94,7 +94,8 @@ def _bits(xs):
 
 SPECIAL = [5e-324, 1e-323, 1.5e-323, 2.2250738585072014e-308, 2.225073858507201e-308, 1.7976931348623157e308, 1e23, 0.0, -0.0,
            9007199254740991.0, 9007199254740992.0, 9007199254740993.0, 9007199254740994.0, 9007199254740996.0,
-           0.1, 0.3, 2.5, 123456.0, 1234567.0, 1e-5, 1e-4, 0.125, 0.375, 3.5, -2.5] + \
+           0.1, 0.3, 2.5, 123456.0, 1234567.0, 1e-5, 1e-4, 0.125, 0.375, 3.5, -2.5,
+           5e-323, 6e-323, 7e-323, 8e-323, 9e-323, 1e-322] + \
           [10.0 ** k for k in range(-30, 31)] + [float(f"1e{k}") for k in range(-30, 31)]
 
 

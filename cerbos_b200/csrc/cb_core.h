@@ -3489,20 +3489,16 @@ CB_HD const uint64_t *list_ptr(const TableView t, const BatchView &b, uint64_t v
 CB_HD bool scalar_eq64(uint64_t x, uint64_t y) {
     return (v64_tag(x) == 0 && v64_tag(y) == 0) ? u2d(x) == u2d(y) : x == y;
 }
-template <typename Cols>
-CB_HD uint64_t term_operand(const TableView t, const BatchView &b, const Cols &cols, uint32_t pid, uint32_t kind, uint32_t v, uint32_t aux) {
+// x[aux] (operand kind SLOT_ELEM)
+CB_HD uint64_t elem_operand(const TableView t, const BatchView &b, uint64_t x, uint32_t aux) {
     const uint64_t kErr = (uint64_t)(CB_V64_BOX_BASE | CB_V64_ERROR) << 48;
-    if (kind == CB_OPK_CONST) return ldg(t.consts_v64() + v);
-    if (kind == CB_OPK_PID) return ((uint64_t)(CB_V64_BOX_BASE | CB_V64_STRING) << 48) | pid;
-    uint64_t x = cols.slot(v);
-    if (kind == CB_OPK_SLOT) return x;
-    uint32_t tx = v64_tag(x);
-    if (kind == CB_OPK_SLOT_ELEM) {
-        if (tx != CB_V64_LIST) return kErr;                       // map[int] / scalar[int]: no such key / overload
-        const uint64_t *p = list_ptr(t, b, x);
-        return aux < (uint32_t)ldg(p) ? ldg(p + 1 + aux) : kErr;   // index out of bounds is an error
-    }
-    // SLOT_SIZE -> double (the compare against an int constant is exact for these magnitudes)
+    if (v64_tag(x) != CB_V64_LIST) return kErr;                   // map[int] / scalar[int]: no such key / overload
+    const uint64_t *p = list_ptr(t, b, x);
+    return aux < (uint32_t)ldg(p) ? ldg(p + 1 + aux) : kErr;       // index out of bounds is an error
+}
+// size(x) (operand kind SLOT_SIZE) -> double (the compare against an int constant is exact for these magnitudes)
+CB_HD uint64_t size_operand(const TableView t, const BatchView &b, uint64_t x) {
+    const uint32_t tx = v64_tag(x);
     if (tx == CB_V64_LIST || tx == CB_V64_MAP) return d2u((double)(uint32_t)ldg(list_ptr(t, b, x)));
     if (tx == CB_V64_STRING) {
         StrRef s = str_ref(t, b, x);
@@ -3510,7 +3506,15 @@ CB_HD uint64_t term_operand(const TableView t, const BatchView &b, const Cols &c
         for (uint32_t i = 0; i < s.len; i++) k += (ldg(s.p + i) & 0xC0) != 0x80;
         return d2u((double)k);
     }
-    return kErr;
+    return (uint64_t)(CB_V64_BOX_BASE | CB_V64_ERROR) << 48;
+}
+template <typename Cols>
+CB_HD uint64_t term_operand(const TableView t, const BatchView &b, const Cols &cols, uint32_t pid, uint32_t kind, uint32_t v, uint32_t aux) {
+    if (kind == CB_OPK_CONST) return ldg(t.consts_v64() + v);
+    if (kind == CB_OPK_PID) return ((uint64_t)(CB_V64_BOX_BASE | CB_V64_STRING) << 48) | pid;
+    uint64_t x = cols.slot(v);
+    if (kind == CB_OPK_SLOT) return x;
+    return kind == CB_OPK_SLOT_ELEM ? elem_operand(t, b, x, aux) : size_operand(t, b, x);
 }
 // shape-specialised term kernels (bytecode._specialize_term): straight-line code, same results as the generic term
 CB_HD bool v64_bad(uint64_t x) { return ((uint32_t)(x >> 48) & 0xFFFEu) == (CB_V64_BOX_BASE | CB_V64_ABSENT); }   // ABSENT or ERROR
@@ -3558,6 +3562,44 @@ CB_HD int in_const_tri(uint64_t x, bool &slow, E... elems) {
     ((found |= scalar_eq64(x, (uint64_t)elems)), ...);
     return found ? TRI_T : TRI_F;
 }
+// the HAS, CMP and STARTS / ENDS / CONTAINS branches of term_tri() on operand values (also called directly by the
+// unique-condition evaluators, cb_specialize.h: generate_uc)
+CB_HD int has_tri(uint64_t x) {
+    const uint32_t tx = v64_tag(x);
+    return tx == CB_V64_ERROR ? TRI_E : (tx != CB_V64_ABSENT);
+}
+CB_HD int cmp_tri(uint32_t ci, uint64_t x, uint64_t y, bool &slow) {
+    const uint32_t tx = v64_tag(x), ty = v64_tag(y);
+    if (v64_bad(x) || v64_bad(y)) return TRI_E;
+    if (tx == 0 && ty == 0) {
+        const double dx = u2d(x), dy = u2d(y);
+        if (ci == 0) return dx == dy;
+        if (dx != dx || dy != dy) return TRI_E;
+        return ci == 2 ? dx < dy : ci == 3 ? dx <= dy : ci == 4 ? dx > dy : dx >= dy;
+    }
+    if (ci == 0 && tx <= CB_V64_STRING && ty <= CB_V64_STRING) return x == y;   // null / bool / interned string / mixed
+    if (ci != 0 && tx != ty) return TRI_E;                                       // no ordering across types
+    slow = true;                                                                 // containers, string ordering, ints
+    return TRI_E;
+}
+CB_HD int str_tri(const TableView t, const BatchView &b, uint32_t op, uint64_t x, uint64_t y) {
+    if (v64_tag(x) != CB_V64_STRING || v64_tag(y) != CB_V64_STRING) return TRI_E;
+    const StrRef a = str_ref(t, b, x), c = str_ref(t, b, y);
+    if (c.len > a.len) return TRI_F;
+    if (op == CB_TERM_CONTAINS) {
+        bool hit = false;
+        for (uint32_t o = 0; o + c.len <= a.len; o++) {
+            bool eq = true;
+            for (uint32_t j = 0; j < c.len; j++) eq &= ldg(a.p + o + j) == ldg(c.p + j);
+            hit |= eq;
+        }
+        return hit;
+    }
+    const uint8_t *ap = op == CB_TERM_STARTS ? a.p : a.p + (a.len - c.len);
+    bool eq = true;
+    for (uint32_t j = 0; j < c.len; j++) eq &= ldg(ap + j) == ldg(c.p + j);
+    return eq;
+}
 // One term {op | flags<<8 | xk<<16 | yk<<24, x, y, xa | ya<<16} -> TRI_T / TRI_F / TRI_E; `slow` is raised for operands
 // this path cannot decide exactly.  Force-inlined: called with a compile-time constant `w` (run-time specialised
 // kernels, cb_specialize.h) the switch, the operand kinds and the slot indices all fold away.
@@ -3578,21 +3620,12 @@ CB_HD int term_tri(const TableView t, const BatchView &b, const Cols &cols, uint
         const uint64_t x = term_operand(t, b, cols, pid, xk, w.y, w.w & 0xFFFF);
         const uint64_t y = op == CB_TERM_HAS ? 0 : term_operand(t, b, cols, pid, yk, w.z, w.w >> 16);
         const uint32_t tx = v64_tag(x), ty = v64_tag(y);
-        const bool xerr = tx == CB_V64_ABSENT || tx == CB_V64_ERROR, yerr = ty == CB_V64_ABSENT || ty == CB_V64_ERROR;
         if (op == CB_TERM_HAS) {
-            tri = tx == CB_V64_ERROR ? TRI_E : (tx != CB_V64_ABSENT);
-        } else if (xerr || yerr) {
-            tri = TRI_E;
+            tri = has_tri(x);
         } else if (op == CB_TERM_CMP) {
-            const uint32_t ci = flags & CB_TERM_CI_MASK;
-            if (tx == 0 && ty == 0) {
-                const double dx = u2d(x), dy = u2d(y);
-                if (ci == 0) tri = dx == dy;
-                else if (dx != dx || dy != dy) tri = TRI_E;
-                else tri = ci == 2 ? dx < dy : ci == 3 ? dx <= dy : ci == 4 ? dx > dy : dx >= dy;
-            } else if (ci == 0 && tx <= CB_V64_STRING && ty <= CB_V64_STRING) tri = x == y;   // null / bool / interned string / mixed
-            else if (ci != 0 && tx != ty) tri = TRI_E;                                         // no ordering across types
-            else slow = true;                                                                  // containers, string ordering, ints
+            tri = cmp_tri(flags & CB_TERM_CI_MASK, x, y, slow);
+        } else if (v64_bad(x) || v64_bad(y)) {
+            tri = TRI_E;
         } else if (op == CB_TERM_IN) {
             if (ty != CB_V64_LIST || tx > CB_V64_STRING) slow = true;   // maps, container members: out of line
             else {
@@ -3607,25 +3640,7 @@ CB_HD int term_tri(const TableView t, const BatchView &b, const Cols &cols, uint
                 tri = found;
             }
         } else if (op == CB_TERM_STARTS || op == CB_TERM_ENDS || op == CB_TERM_CONTAINS) {
-            if (tx != CB_V64_STRING || ty != CB_V64_STRING) tri = TRI_E;
-            else {
-                const StrRef a = str_ref(t, b, x), c = str_ref(t, b, y);
-                if (c.len > a.len) tri = TRI_F;
-                else if (op == CB_TERM_CONTAINS) {
-                    bool hit = false;
-                    for (uint32_t o = 0; o + c.len <= a.len; o++) {
-                        bool eq = true;
-                        for (uint32_t j = 0; j < c.len; j++) eq &= ldg(a.p + o + j) == ldg(c.p + j);
-                        hit |= eq;
-                    }
-                    tri = hit;
-                } else {
-                    const uint8_t *ap = op == CB_TERM_STARTS ? a.p : a.p + (a.len - c.len);
-                    bool eq = true;
-                    for (uint32_t j = 0; j < c.len; j++) eq &= ldg(ap + j) == ldg(c.p + j);
-                    tri = eq;
-                }
-            }
+            tri = str_tri(t, b, op, x, y);
         } else {   // INTERSECTS / SUBSET on two lists (cerbos_lib.go:323-431)
             if (tx != CB_V64_LIST || ty != CB_V64_LIST) tri = TRI_E;
             else {
@@ -3650,6 +3665,22 @@ CB_HD int term_tri(const TableView t, const BatchView &b, const Cols &cols, uint
     }
     }
     return tri;
+}
+// The generic term path as the unique-condition evaluators call it, for terms without a register form
+// (cb_specialize.h: generate_uc).
+template <typename Cols>
+CB_HD int uc_term_tri(const TableView t, const BatchView &b, const Cols &cols, uint32_t pid, const U4 w, bool &slow) {
+#ifdef CB_UC_STUB_TERMS   // tools/uc_variants.sh: the generic terms replaced by one register read (wrong results)
+    return (int)(cols.slot(w.y) & 1u);
+#endif
+    return term_tri(t, b, cols, pid, w, slow);
+}
+template <typename Cols>
+CB_HD uint64_t uc_term_operand(const TableView t, const BatchView &b, const Cols &cols, uint32_t pid, uint32_t kind, uint32_t v, uint32_t aux) {
+#ifdef CB_UC_STUB_TERMS
+    return ((uint64_t)(CB_V64_BOX_BASE | CB_V64_STRING) << 48) | (uint32_t)cols.slot(v);   // a string: nothing defers
+#endif
+    return term_operand(t, b, cols, pid, kind, v, aux);
 }
 // ---- register-resident lists (run-time specialised unique-condition kernels) ----------------------------------------
 // Several conditions of a table usually read the same list attribute (principal groups, allowed groups ...).  The
@@ -3738,6 +3769,21 @@ CB_HD ListRegs list_load(const TableView t, const BatchView &b, uint64_t x) {
     }
     if (L.st == 0) L.st = odd ? 2u : 0u;
     return L;
+}
+// size(x) / x[i] from the list registers L = list_load(x): the SLOT_SIZE / SLOT_ELEM operands of term_operand() for
+// every value.  The length is the list header (exact for st 0 and 2); an element is in registers only for st 0.
+CB_HD uint64_t list_size(const TableView t, const BatchView &b, uint64_t x, const ListRegs &L) {
+    if (L.st == 0 || L.st == 2) return d2u((double)L.len);
+    return size_operand(t, b, x);   // absent / error (an error), string, map: not a list
+}
+CB_HD uint64_t list_elem(const TableView t, const BatchView &b, uint64_t x, const ListRegs &L, uint32_t i) {
+    if (L.st == 2) return elem_operand(t, b, x, i);                                    // elements the registers do not hold
+    if (L.st != 0 || i >= L.len) return (uint64_t)(CB_V64_BOX_BASE | CB_V64_ERROR) << 48;  // not a list / out of bounds
+#ifndef CB_LIST_KEYS64
+    return ((uint64_t)kStringTop << 48) | L.e[i];
+#else
+    return L.e[i];   // -0.0 held as +0.0: equal under every compare a term makes
+#endif
 }
 // x in L: the outcome of in_tri() / the IN branch of term_tri() for every input this form decides, `slow` otherwise
 CB_HD int list_in_tri(uint64_t x, const ListRegs &L, bool &slow) {

@@ -493,6 +493,9 @@ inline UcSource generate_uc(const uint8_t *uc_image, const uint32_t *off, uint32
         default:
             use_slot(xk, w[1]);
             if (op != CB_TERM_HAS) use_slot(yk, w[2]);
+            // size() is read from the list registers: the slot becomes a list slot
+            if (xk == CB_OPK_SLOT_SIZE && w[1] < ns) slot_list[w[1]] = true;
+            if (op != CB_TERM_HAS && yk == CB_OPK_SLOT_SIZE && w[2] < ns) slot_list[w[2]] = true;
             if (op == CB_TERM_IN && yk == CB_OPK_SLOT && w[2] < ns) { slot_list[w[2]] = true; form[q] = 'L'; }
             if ((op == CB_TERM_INTERSECTS || op == CB_TERM_SUBSET) && xk == CB_OPK_SLOT && yk == CB_OPK_SLOT && w[1] < ns && w[2] < ns) {
                 slot_list[w[1]] = slot_list[w[2]] = true;
@@ -530,19 +533,44 @@ inline UcSource generate_uc(const uint8_t *uc_image, const uint32_t *off, uint32
             mask_of[q] = k;
         }
     auto sl = [](uint32_t v) { return "cols.slot(" + std::to_string(v) + "u)"; };
+    // an operand as a value held in registers ("": none -- the generic term path loads it)
+    auto operand = [&](uint32_t kind, uint32_t v, uint32_t aux) -> std::string {
+        if (kind == CB_OPK_CONST) return hex64(consts[v]);
+        if (kind == CB_OPK_PID) return "(((uint64_t)(CB_V64_BOX_BASE | CB_V64_STRING) << 48) | pid)";
+        if (v >= ns) return "";
+        if (kind == CB_OPK_SLOT) return sl(v);
+        const std::string l = "cols.l" + std::to_string(v);
+        if (kind == CB_OPK_SLOT_SIZE && slot_list[v]) return "list_size(t, b, " + sl(v) + ", " + l + ")";
+        if (kind == CB_OPK_SLOT_ELEM && slot_list[v] && aux < 8) return "list_elem(t, b, " + sl(v) + ", " + l + ", " + std::to_string(aux) + "u)";   // CB_LC
+        return "";
+    };
     auto term_code = [&](uint32_t q) -> std::string {
         const uint32_t *w = terms[q].data();
-        const uint32_t op = w[0] & 0xFF, xk = (w[0] >> 16) & 0xFF;
+        const uint32_t op = w[0] & 0xFF, flags = (w[0] >> 8) & 0xFF, xk = (w[0] >> 16) & 0xFF, yk = w[0] >> 24;
+        const bool kinds = op <= CB_TERM_SUBSET;   // the generic shapes name their operands' kinds
+        const std::string x = kinds ? operand(xk, w[1], w[3] & 0xFFFFu) : "", y = kinds && op != CB_TERM_HAS ? operand(yk, w[2], w[3] >> 16) : "";
         if (form[q] == 'P') return "strpred_tri(b, " + sl(w[1]) + ", " + std::to_string(pred_of[q]) + "u)";
         if (form[q] == 'L') {
             if (op == CB_TERM_IN_CS) return "list_in_tri(" + hex64(consts[w[1]]) + ", cols.l" + std::to_string(w[2]) + ", slow)";
             if (op == CB_TERM_IN_SS) return "list_in_tri(" + sl(w[1]) + ", cols.l" + std::to_string(w[2]) + ", slow)";
             if (op == CB_TERM_IN)
-                return "list_in_tri(term_operand(t, b, cols, pid, " + hex(xk) + ", " + hex(w[1]) + ", " + hex(w[3] & 0xFFFFu) + "), cols.l" + std::to_string(w[2]) + ", slow)";
+                return "list_in_tri(" + (!x.empty() ? x : "uc_term_operand(t, b, cols, pid, " + hex(xk) + ", " + hex(w[1]) + ", " + hex(w[3] & 0xFFFFu) + ")") +
+                       ", cols.l" + std::to_string(w[2]) + ", slow)";
             const std::string a = std::to_string(mask_of[q].first), bb = std::to_string(mask_of[q].second);
             return std::string("list_set_tri(") + (op == CB_TERM_SUBSET ? "true" : "false") + ", cols.l" + a + ", cols.l" + bb + ", m" + a + "_" + bb + ", slow)";
         }
-        return term_expr(w, consts, theap);
+        // the shapes term_tri() folds to, and the generic shapes over operands held in registers: the same helpers, called directly
+        if (w[1] < ns && w[2] < ns) {
+            if (op == CB_TERM_EQ_SS) return "eq_tri(" + sl(w[1]) + ", " + sl(w[2]) + ", slow)";
+            if (op == CB_TERM_ORD_SS) return "ord_tri(" + hex(flags & CB_TERM_CI_MASK) + ", " + sl(w[1]) + ", " + sl(w[2]) + ", slow)";
+        }
+        if (op == CB_TERM_EQ_SP && w[1] < ns) return "eq_tri(" + sl(w[1]) + ", " + operand(CB_OPK_PID, 0, 0) + ", slow)";
+        if (op == CB_TERM_HAS && !x.empty()) return "has_tri(" + x + ")";
+        if (op == CB_TERM_CMP && !x.empty() && !y.empty()) return "cmp_tri(" + hex(flags & CB_TERM_CI_MASK) + ", " + x + ", " + y + ", slow)";
+        if ((op == CB_TERM_STARTS || op == CB_TERM_ENDS || op == CB_TERM_CONTAINS) && !x.empty() && !y.empty())
+            return "str_tri(t, b, " + std::to_string(op) + "u, " + x + ", " + y + ")";
+        const std::string e = term_expr(w, consts, theap);
+        return e.compare(0, 9, "term_tri(") == 0 ? "uc_" + e : e;
     };
     // Slots read by the flat terms live in registers (all loads in flight at once); slots only the leaf programs read --
     // and every slot once the table reads more than kMaxRegSlots of them -- are loaded where they are used (L1-allocating loads).

@@ -16,6 +16,7 @@ run default X=1
 run stub_walk CERBOS_B200_SPEC_DEFS=-DCB_UC_STUB_WALK
 run stub_lists CERBOS_B200_SPEC_DEFS=-DCB_UC_STUB_LISTS
 run stub_strpred CERBOS_B200_SPEC_DEFS=-DCB_UC_STUB_STRPRED
+run stub_terms CERBOS_B200_SPEC_DEFS=-DCB_UC_STUB_TERMS
 run keys64 CERBOS_B200_SPEC_DEFS=-DCB_LIST_KEYS64
 run blocks3 CERBOS_B200_SPEC_UC_BLOCKS=3
 run blocks4 CERBOS_B200_SPEC_UC_BLOCKS=4

@@ -24,6 +24,7 @@
 #include "cb_uc.h"
 #include "cb_encode.h"
 #include "cb_narrow.h"
+#include "cb_host.h"
 #include "cb_embed.inc"
 #include "cerbos_b200.h"
 
@@ -34,7 +35,6 @@ constexpr int kThreads = cbk::kThreads;
 #define CB_MIN_BLOCKS 4   // resident CTAs / SM the check kernel is register-budgeted for (64 registers per thread)
 #endif
 constexpr uint32_t kMaxStageBytes = 96 * 1024;   // table images up to this size are TMA-staged into shared memory
-constexpr int kMaxSec = 32;
 constexpr uint32_t kMaxTilesSmem = 56 * 1024;    // image + two column-tile stages: keeps CB_MIN_BLOCKS CTAs resident per SM
 
 using cbk::TableDesc;
@@ -476,7 +476,7 @@ struct cgpu_table {
     uint32_t spec_n_strpred = 0;   // string predicates the specialised unique-condition kernel reads from the per-string pre-pass
     std::string spec_note;
     // unique-condition image (cb_uc.h): compact copy of the table for tables whose blocks differ in shape
-    uint64_t sec_len[kMaxSec]{};
+    uint64_t sec_len[cbhost::kMaxSec]{};
     std::vector<cgpu_table *> peer_tables;   // the same table on the other devices of a multi-device context (owned)
     cbuc::Image uc;
     uint8_t *d_uc_image = nullptr;
@@ -487,106 +487,8 @@ struct cgpu_table {
 
 namespace {
 
-int parse_blob(const void *blob, size_t len, TableDesc *d, uint32_t *meta, uint64_t *sec_len = nullptr) {
-    if (!blob || len < sizeof(cb_blob_header)) return fail(CGPU_ERR_INVALID, "table blob too small");
-    const cb_blob_header *h = static_cast<const cb_blob_header *>(blob);
-    if (h->magic != CB_MAGIC) return fail(CGPU_ERR_INVALID, "table blob: bad magic");
-    if (h->version != CB_VERSION) return fail(CGPU_ERR_INVALID, "table blob: version %u, library expects %u", h->version, CB_VERSION);
-    if (h->total_bytes > len || sizeof(cb_blob_header) + (size_t)h->n_sections * sizeof(cb_section_desc) > len)
-        return fail(CGPU_ERR_INVALID, "table blob truncated");
-    const cb_section_desc *sd = reinterpret_cast<const cb_section_desc *>(static_cast<const char *>(blob) + sizeof(cb_blob_header));
-    memset(d, 0, sizeof(*d));
-    uint64_t image_end = 0;
-    bool seen[kMaxSec] = {false};
-    for (uint32_t i = 0; i < h->n_sections; i++) {
-        if (sd[i].offset > len || sd[i].n_bytes > len - sd[i].offset || (sd[i].offset & 15)) return fail(CGPU_ERR_INVALID, "table blob: bad section %u", sd[i].id);
-        if (sd[i].id == CB_SEC_MANIFEST) continue;   // host-only
-        if (sd[i].id >= kMaxSec) continue;
-        if (sd[i].offset > 0xFFFFFFF0ull) return fail(CGPU_ERR_INVALID, "table blob too large");
-        d->lay.off[sd[i].id] = (uint32_t)sd[i].offset;
-        if (sec_len) sec_len[sd[i].id] = sd[i].n_bytes;
-        seen[sd[i].id] = true;
-        uint64_t end = (sd[i].offset + sd[i].n_bytes + 15) & ~15ull;
-        if (end > image_end) image_end = end;
-        if (sd[i].id == CB_SEC_META) {
-            if (sd[i].n_bytes < CB_META_WORDS * 4) return fail(CGPU_ERR_INVALID, "table blob: short META");
-            memcpy(meta, static_cast<const char *>(blob) + sd[i].offset, CB_META_WORDS * 4);
-        }
-    }
-    for (int id = CB_SEC_META; id <= CB_SEC_DR_NAME_STR; id++)
-        if (!seen[id]) return fail(CGPU_ERR_INVALID, "table blob: missing section %d", id);
-    if (image_end > 0xFFFFFFF0ull) return fail(CGPU_ERR_INVALID, "table blob too large");
-    if (image_end > len) image_end = len;   // the last device section may end unaligned at the end of the blob (sections themselves are bounds-checked above)
-    d->lay.image_bytes = (uint32_t)image_end;
-    d->lay.nV = meta[CB_META_N_VERSIONS]; d->lay.nRP = meta[CB_META_N_RESPATS]; d->lay.nS = meta[CB_META_N_SCOPES];
-    d->lay.nP = meta[CB_META_N_PRINCIPALS]; d->lay.nR = meta[CB_META_N_ROLES]; d->lay.nAP = meta[CB_META_N_APATS];
-    d->lay.nT = meta[CB_META_N_STRINGS]; d->lay.n_slots = meta[CB_META_N_SLOTS]; d->lay.n_rows = meta[CB_META_N_ROWS] ? meta[CB_META_N_ROWS] : 1;
-    d->lay.has_role_policies = meta[CB_META_HAS_ROLE_POLICIES]; d->lay.has_parent_roles = meta[CB_META_HAS_PARENT_ROLES];
-    d->lay.has_principal_policies = meta[CB_META_HAS_PRINCIPAL_POLICIES];
-    d->lay.uses_runtime = meta[CB_META_USES_RUNTIME];
-    if (sec_len) {
-        struct { int id; uint64_t need; } chk[] = {
-            {CB_SEC_SCOPE_PARENT, 4ull * d->lay.nS}, {CB_SEC_SCOPE_FLAGS, 4ull * d->lay.nS},
-            {CB_SEC_RES_BLOCK_MAP, 4ull * d->lay.nV * d->lay.nRP * d->lay.nS}, {CB_SEC_RES_EXISTS, 1ull * d->lay.nV * d->lay.nRP * d->lay.nS},
-            {CB_SEC_PRIN_BLOCK_MAP, 4ull * d->lay.nV * d->lay.nP * d->lay.nS}, {CB_SEC_PRIN_EXISTS, 1ull * d->lay.nV * d->lay.nS},
-            {CB_SEC_BLOCKS, 16ull * meta[CB_META_N_BLOCKS]}, {CB_SEC_ROWS, 16ull * meta[CB_META_N_ROWS]}, {CB_SEC_CONDS, 16ull * meta[CB_META_N_CONDS]},
-            {CB_SEC_CODE, 8ull * meta[CB_META_N_CODE]}, {CB_SEC_CONSTS, 16ull * meta[CB_META_N_CONSTS]}, {CB_SEC_CONSTS_V64, 8ull * meta[CB_META_N_CONSTS]},
-            {CB_SEC_STR_OFF, 4ull * (d->lay.nT + 1)}, {CB_SEC_THEAP, 8ull * meta[CB_META_THEAP_WORDS]},
-            {CB_SEC_BLOCK_SLOTS_OFF, 4ull * (meta[CB_META_N_BLOCKS] + 1)}, {CB_SEC_DR_OFF, 4ull * (meta[CB_META_N_BLOCKS] + 1)},
-            {CB_SEC_DR_NAME_STR, 4ull * meta[CB_META_N_DR_NAMES]},
-        };
-        for (const auto &c : chk)
-            if (sec_len[c.id] < c.need) return fail(CGPU_ERR_INVALID, "table blob: section %d holds %llu bytes, META needs %llu", c.id, (unsigned long long)sec_len[c.id], (unsigned long long)c.need);
-    }
-    if (meta[CB_META_MAX_STACK] > CB_MAX_STACK || meta[CB_META_MAX_LOOP_DEPTH] > CB_MAX_LOOP_DEPTH || meta[CB_META_N_VARS] > CB_MAX_VARS)
-        return fail(CGPU_ERR_INVALID, "table blob needs a deeper interpreter than this build provides");
-    return CGPU_OK;
-}
-
-// Validates the batch against the table and fills the device view (pointers are used as given).
-int make_batch_view(const cgpu_table *t, const cgpu_batch *b, uint64_t first, uint64_t count, cb::BatchView *v) {
-    if (!b || b->n_columns < CGPU_N_COLUMNS || !b->columns || !b->column_bytes) return fail(CGPU_ERR_INVALID, "batch: expected %d columns", CGPU_N_COLUMNS);
-    const uint64_t N = b->n_requests;
-    if (N == 0) return fail(CGPU_ERR_INVALID, "batch: empty");
-    const size_t *cb_ = b->column_bytes;
-    if (cb_[CGPU_COL_HDR0] < N * 16 || cb_[CGPU_COL_HDR1] < N * 8) return fail(CGPU_ERR_INVALID, "batch: header columns too small");
-    if (cb_[CGPU_COL_ROLES] % (4 * N) != 0) return fail(CGPU_ERR_INVALID, "batch: roles column is not a multiple of n_requests");
-    uint32_t role_cols = (uint32_t)(cb_[CGPU_COL_ROLES] / (4 * N));
-    if (role_cols == 0 || role_cols > CB_MAX_ROLE_COLS) return fail(CGPU_ERR_INVALID, "batch: %u role columns (supported 1..%d)", role_cols, CB_MAX_ROLE_COLS);
-    if (cb_[CGPU_COL_SLOTS] < (size_t)8 * t->desc.lay.n_slots * N) return fail(CGPU_ERR_INVALID, "batch: slot columns too small for the table's %u slots", t->desc.lay.n_slots);
-    uint32_t n_asets = (uint32_t)(cb_[CGPU_COL_ASET_K] / 4);
-    if (n_asets == 0) return fail(CGPU_ERR_INVALID, "batch: no action sets");
-    uint32_t km = b->max_actions ? b->max_actions : 1;
-    uint32_t kc = 64 / role_cols;
-    if (kc > km) kc = km;
-    uint32_t n_pass = (km + kc - 1) / kc;
-    uint32_t nAP = t->desc.lay.nAP ? t->desc.lay.nAP : 1;
-    if (cb_[CGPU_COL_ASET_SPREAD] < (size_t)8 * n_pass * n_asets * nAP) return fail(CGPU_ERR_INVALID, "batch: aset_spread too small");
-    if (cb_[CGPU_COL_ROW_AM] < (size_t)8 * n_pass * n_asets * t->desc.lay.n_rows) return fail(CGPU_ERR_INVALID, "batch: row_am too small");
-    for (int i = 0; i < CGPU_N_COLUMNS; i++)
-        if (!b->columns[i]) return fail(CGPU_ERR_INVALID, "batch: column %d is null", i);
-    v->hdr0 = static_cast<const cb_hdr0 *>(b->columns[CGPU_COL_HDR0]);
-    v->hdr1 = static_cast<const cb_hdr1 *>(b->columns[CGPU_COL_HDR1]);
-    v->roles = static_cast<const uint32_t *>(b->columns[CGPU_COL_ROLES]);
-    v->slots = static_cast<const uint64_t *>(b->columns[CGPU_COL_SLOTS]);
-    v->heap = static_cast<const uint64_t *>(b->columns[CGPU_COL_HEAP]);
-    v->bstr_off = static_cast<const uint32_t *>(b->columns[CGPU_COL_BSTR_OFF]);
-    v->bstr_bytes = static_cast<const uint8_t *>(b->columns[CGPU_COL_BSTR_BYTES]);
-    v->class_off = static_cast<const uint32_t *>(b->columns[CGPU_COL_CLASS_OFF]);
-    v->class_pats = static_cast<const uint32_t *>(b->columns[CGPU_COL_CLASS_PATS]);
-    v->aset_k = static_cast<const uint32_t *>(b->columns[CGPU_COL_ASET_K]);
-    v->aset_spread = static_cast<const uint64_t *>(b->columns[CGPU_COL_ASET_SPREAD]);
-    v->row_am = static_cast<const uint64_t *>(b->columns[CGPU_COL_ROW_AM]);
-    v->n_rows = t->desc.lay.n_rows;
-    v->stride = N; v->first = first; v->count = count;
-    v->role_cols = role_cols; v->n_asets = n_asets; v->kc = kc; v->n_pass = n_pass; v->max_actions = km;
-    v->kbytes = (km + 7) / 8; v->flags = b->flags; v->now = b->now_unix_nanos;
-    cb::finish_batch_view(*v);
-    v->n_bstr = cb_[CGPU_COL_BSTR_OFF] >= 4 ? (uint32_t)(cb_[CGPU_COL_BSTR_OFF] / 4 - 1) : 0;
-    v->heap_words = cb_[CGPU_COL_HEAP] / 8;
-    return CGPU_OK;
-}
-
+// A shared host check (cb_host.h) that failed: its message becomes the error of the call.
+int invalid(const std::string &why) { return why.empty() ? CGPU_OK : fail(CGPU_ERR_INVALID, "%s", why.c_str()); }
 
 // ---------------------------------------------------------------------------------------------- run-time specialisation
 // NVRTC is loaded lazily with dlopen: a host without it simply keeps the ahead-of-time (generic) kernels.
@@ -708,11 +610,6 @@ void cache_write(const std::string &path, const std::vector<char> &data) {
 enum SpecForm { SPEC_NONE = 0, SPEC_SHAPES = 1, SPEC_UC = 2 };
 constexpr uint32_t kUcMaxSmem = 72 * 1024;   // compact image + merged rows: three CTAs / SM at least
 
-// Resource-policy-only tables (no principal / role policies, no parent roles) whose kinds resolve without resource globs:
-// the only tables a lean kernel body can evaluate.
-bool lean_table(const cb::TableLayout &lay, const uint32_t *meta) {
-    return !lay.has_principal_policies && !lay.has_role_policies && !lay.has_parent_roles && meta[CB_META_DIRECT_KINDS];
-}
 // Shared memory of a staged unique-condition launch: the compact image, then one 16-byte merged row per (action set, row).
 uint64_t uc_smem_bytes(const cbuc::Image &uc, uint64_t n_pk) { return (((uint64_t)uc.lay.image_bytes + 127) & ~127ull) + 16 * n_pk; }
 // Whether the staged unique-condition kernel fits with n_pk merged rows.  With one (the default) it is the question whether
@@ -724,7 +621,7 @@ SpecForm spec_generate(const uint8_t *image, const cb::TableLayout &lay, const u
     *n_strpred = 0;
     if (n_atoms) *n_atoms = 0;
     // the specialised kernels are lean bodies: a table that can never take a lean kernel needs none
-    if (!lean_table(lay, meta)) {
+    if (!cbhost::lean_table(lay, meta)) {
         *why = "table is not lean-eligible (principal / role policies, parent roles or resource globs): general kernel only";
         return SPEC_NONE;
     }
@@ -909,8 +806,6 @@ LaunchPlan plan_launch(const cgpu_ctx &ctx, const cgpu_table &t, const cb::Batch
     const cb::TableLayout &lay = t.desc.lay;
     LaunchPlan p;
     p.stage = !ctx.force_no_stage && lay.image_bytes <= kMaxStageBytes;
-    uint32_t rcp = 1;
-    while (rcp < bv.role_cols) rcp <<= 1;
     // the kernels compiled for the table are used once they are loaded: a launch never waits for the compile
     const bool spec_ready = t.spec_state.load(std::memory_order_acquire) == 1;
     const bool uc_spec_ready = spec_ready && t.spec_uc_global != nullptr;
@@ -918,15 +813,12 @@ LaunchPlan plan_launch(const cgpu_ctx &ctx, const cgpu_table &t, const cb::Batch
     // (leaf programs as straight-line code) is loaded: the lean body would defer nearly every request to the one-CTA-per-SM
     // drain launch.  Such launches go to the general kernel at full occupancy instead.
     const bool mostly_programs = t.uc.ok && !uc_spec_ready && 2 * (uint64_t)t.uc.n_gids_flat < t.uc.n_gids;
-    // The lean body applies to lean tables when the (action x role column) pair masks fit 32 bits and the role table fits 64 bits.
-    p.lean = !ctx.force_general && !mostly_programs && bv.n_pass == 1 && (uint64_t)bv.max_actions * bv.role_cols <= 32 && bv.kbytes <= 4 &&
-             lean_table(lay, t.meta) && (uint64_t)lay.nR * rcp <= 64;
+    p.lean = !ctx.force_general && !mostly_programs && cbhost::lean_eligible(lay, t.meta, bv);
     // Unique-condition kernels: lean-eligible tables with <= 63 distinct conditions whose blocks differ in shape
     // (with one shape the per-shape specialised tile kernel is the better fit).  Index order, no clustering.
     // (an image with condition programs or index-form rows is only good for the specialised kernel: cbuc::Image::needs_spec)
     const uint64_t n_pk = (uint64_t)bv.n_asets * lay.n_rows;   // merged rows: one per (action set, row)
-    p.uc = p.lean && t.uc.ok && (uc_spec_ready || !t.uc.needs_spec()) && t.d_uc_image && bv.count < (1ull << 32) && n_pk < (1ull << 31) &&
-           (uint64_t)(lay.nR + 1) * rcp <= 64 &&
+    p.uc = p.lean && cbhost::uc_eligible(lay, t.uc, bv) && (uc_spec_ready || !t.uc.needs_spec()) && t.d_uc_image &&
            (ctx.uc_mode == 1 || (ctx.uc_mode != 0 && ctx.cluster_mode != 1 && t.meta[CB_META_BLOCK_SHAPES] > 1));   // CERBOS_B200_CLUSTER=1 keeps the clustered path reachable
     // Clustering pays when the policy blocks differ in shape (rows / conditions): with a single shape every lane runs
     // the same control flow in index order already and the coalesced column loads are worth more.
@@ -1211,7 +1103,7 @@ int cgpu_table_load(cgpu_ctx *ctx, const void *blob, size_t len, cgpu_table **ou
     cgpu_table *t = new (std::nothrow) cgpu_table();
     if (!t) return fail(CGPU_ERR_INVALID, "out of memory");
     t->ctx = ctx;
-    int rc = parse_blob(blob, len, &t->desc, t->meta, t->sec_len);
+    int rc = invalid(cbhost::parse_blob(blob, len, &t->desc.lay, t->meta, t->sec_len));
     if (rc != CGPU_OK) { delete t; return rc; }
     t->uc = cbuc::build(static_cast<const uint8_t *>(blob), t->desc.lay.off, t->sec_len, t->meta, t->desc.lay);
     cudaError_t e = cudaSetDevice(ctx->device);
@@ -1269,16 +1161,16 @@ void cgpu_table_release(cgpu_table *t) {
 int cgpu_table_compile_check(const void *blob, size_t len, size_t *cubin_bytes) {
     if (!blob || !cubin_bytes) return fail(CGPU_ERR_INVALID, "cgpu_table_compile_check: null argument");
     *cubin_bytes = 0;
-    TableDesc d;
+    cb::TableLayout lay;
     uint32_t meta[CB_META_WORDS];
-    uint64_t sec_len[kMaxSec] = {0};
-    int rc = parse_blob(blob, len, &d, meta, sec_len);
+    uint64_t sec_len[cbhost::kMaxSec] = {0};
+    int rc = invalid(cbhost::parse_blob(blob, len, &lay, meta, sec_len));
     if (rc != CGPU_OK) return rc;
-    const cbuc::Image uc = cbuc::build(static_cast<const uint8_t *>(blob), d.lay.off, sec_len, meta, d.lay);
+    const cbuc::Image uc = cbuc::build(static_cast<const uint8_t *>(blob), lay.off, sec_len, meta, lay);
     std::vector<char> cubin;
     std::string why;
     uint32_t n_strpred = 0;
-    const SpecForm form = spec_compile(static_cast<const uint8_t *>(blob), d.lay, meta, uc, &cubin, &why, &n_strpred);
+    const SpecForm form = spec_compile(static_cast<const uint8_t *>(blob), lay, meta, uc, &cubin, &why, &n_strpred);
     if (form == SPEC_NONE) {
         g_err = why;
         return why.rfind("NVRTC compile failed", 0) == 0 ? CGPU_ERR_CUDA : CGPU_OK;   // not qualifying is not an error
@@ -1369,7 +1261,7 @@ int cgpu_check_device(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *dev_
     if (!ctx || !t || !dev_batch || !dev_bitmap_out) return fail(CGPU_ERR_INVALID, "cgpu_check_device: null argument");
     if (t->ctx != ctx) return fail(CGPU_ERR_INVALID, "table belongs to another context");
     cb::BatchView bv;
-    int rc = make_batch_view(t, dev_batch, 0, dev_batch->n_requests, &bv);
+    int rc = invalid(cbhost::make_batch_view(t->desc.lay, dev_batch, 0, dev_batch->n_requests, &bv));
     if (rc != CGPU_OK) return rc;
     CUDA_TRY(cudaSetDevice(ctx->device));
     cudaStream_t s = static_cast<cudaStream_t>(cuda_stream);   // NULL = the legacy default stream
@@ -1427,7 +1319,7 @@ int cgpu_check_device_gather(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batc
     if (g->n_ranks == 0 || g->n_ranks > cb::CB_MAX_GATHER || g->my_rank >= g->n_ranks || g->step == 0)
         return fail(CGPU_ERR_INVALID, "cgpu_check_device_gather: 1..%d ranks, my_rank < n_ranks, step > 0", cb::CB_MAX_GATHER);
     cb::BatchView bv;
-    int rc = make_batch_view(t, dev_batch, 0, dev_batch->n_requests, &bv);
+    int rc = invalid(cbhost::make_batch_view(t->desc.lay, dev_batch, 0, dev_batch->n_requests, &bv));
     if (rc != CGPU_OK) return rc;
     if (bv.kbytes > 8) return fail(CGPU_ERR_UNSUPPORTED, "fused gather supports up to 64 actions per request");
     if ((uint64_t)bv.count * bv.kbytes > g->slice_bytes) return fail(CGPU_ERR_INVALID, "gather slice too small");
@@ -1732,7 +1624,7 @@ int cgpu_check_meta(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch,
     const uint32_t km = batch->max_actions ? batch->max_actions : 1;
     if (N == 0) return CGPU_OK;
     cb::BatchView hv;
-    int rc = make_batch_view(t, batch, 0, N, &hv);
+    int rc = invalid(cbhost::make_batch_view(t->desc.lay, batch, 0, N, &hv));
     if (rc != CGPU_OK) return rc;
     CUDA_TRY(cudaSetDevice(ctx->device));
     // the metadata plane is the cold path (IncludeMeta requests, audit): plain stream-ordered scratch, one launch
@@ -1756,7 +1648,7 @@ int cgpu_check_meta(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch,
     cgpu_batch db = *batch;
     db.columns = dcols;
     cb::BatchView bv;
-    rc = make_batch_view(t, &db, 0, N, &bv);
+    rc = invalid(cbhost::make_batch_view(t->desc.lay, &db, 0, N, &bv));
     if (rc != CGPU_OK) return rc;
     uint8_t *d_eff = dbase + offs[CGPU_N_COLUMNS];
     uint32_t *d_am = reinterpret_cast<uint32_t *>(dbase + offs[CGPU_N_COLUMNS + 1]);
@@ -1803,7 +1695,7 @@ static int check_range(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *bat
     const uint64_t N = batch->n_requests;
     const uint32_t km = batch->max_actions ? batch->max_actions : 1;
     cb::BatchView hv;
-    int rc = make_batch_view(t, batch, 0, N, &hv);   // validates sizes (pointers here are host pointers)
+    int rc = invalid(cbhost::make_batch_view(t->desc.lay, batch, 0, N, &hv));   // validates sizes (pointers here are host pointers)
     if (rc != CGPU_OK) return rc;
     CUDA_TRY(cudaSetDevice(ctx->device));
 
@@ -1865,7 +1757,7 @@ static int check_range(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *bat
     cgpu_batch db = *batch;
     db.columns = dcols;
     cb::BatchView bv;
-    rc = make_batch_view(t, &db, 0, N, &bv);
+    rc = invalid(cbhost::make_batch_view(t->desc.lay, &db, 0, N, &bv));
     if (rc != CGPU_OK) return rc;
     uint8_t *d_effects = dbase + offs[CGPU_N_COLUMNS];
 

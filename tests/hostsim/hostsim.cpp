@@ -10,6 +10,7 @@
 #include "cb_specialize.h"
 #include "cb_uc.h"
 #include "cb_encode.h"
+#include "cb_host.h"
 
 #if defined(HOSTSIM_SPEC_UC)
 #include "spec_gen.inc"   // generated for one table by hostsim_generate_uc: cb::SpecConds (unique-condition form)
@@ -27,92 +28,79 @@ typedef cb::GenericConds HostConds;
 #define HOSTSIM_ENTRY hostsim_check
 #endif
 
-extern "C" { uint64_t hostsim_deferred = 0; }   // requests the lean / unique-condition body left to the general body in the last call
-static bool parse_sections(const void *blob, uint64_t blob_len, uint32_t *off, uint64_t *len) {
-    const cb_blob_header *h = static_cast<const cb_blob_header *>(blob);
-    if (blob_len < sizeof(*h) || h->magic != CB_MAGIC || h->version != CB_VERSION) return false;
-    const cb_section_desc *sd = reinterpret_cast<const cb_section_desc *>(static_cast<const char *>(blob) + sizeof(cb_blob_header));
-    for (uint32_t i = 0; i < h->n_sections; i++) if (sd[i].id < 128) { off[sd[i].id] = (uint32_t)sd[i].offset; len[sd[i].id] = sd[i].n_bytes; }
-    return true;
+extern "C" {
+uint64_t hostsim_deferred = 0;   // requests the lean / unique-condition body left to the general body in the last call
+int hostsim_body = 1;            // the body the last check call ran, by the mode that selects it (1: the general 64-bit body)
+}
+
+// A table and a batch set up the way the library sets them up (cb_host.h)
+struct Setup {
+    const uint8_t *base = nullptr;
+    cb::TableLayout lay;
+    uint32_t meta[CB_META_WORDS];
+    uint64_t sec_len[cbhost::kMaxSec] = {};
+    cb::BatchView b;
+};
+// false: the library would refuse the blob, or (cols given) the batch
+static bool setup(Setup &s, const void *blob, uint64_t blob_len, const void *const *cols = nullptr, const uint64_t *col_bytes = nullptr,
+                  uint64_t n = 0, uint32_t max_actions = 0, int64_t now = 0, uint32_t flags = 0) {
+    s.base = static_cast<const uint8_t *>(blob);
+    if (!cbhost::parse_blob(blob, blob_len, &s.lay, s.meta, s.sec_len).empty()) return false;
+    if (!cols) return true;
+    cgpu_batch batch;
+    batch.n_requests = n; batch.max_actions = max_actions; batch.now_unix_nanos = now; batch.flags = flags;
+    batch.columns = cols; batch.column_bytes = col_bytes; batch.n_columns = CGPU_N_COLUMNS;
+    return cbhost::make_batch_view(s.lay, &batch, 0, n, &s.b).empty();
 }
 
 extern "C" int HOSTSIM_ENTRY(const void *blob, uint64_t blob_len, uint64_t n, uint32_t max_actions, int64_t now, uint32_t flags,
                              const void *const *cols, const uint64_t *col_bytes, uint8_t *bitmap, int mode) {
-    const cb_blob_header *h = static_cast<const cb_blob_header *>(blob);
-    if (blob_len < sizeof(*h) || h->magic != CB_MAGIC || h->version != CB_VERSION) return -1;
-    const cb_section_desc *sd = reinterpret_cast<const cb_section_desc *>(static_cast<const char *>(blob) + sizeof(cb_blob_header));
-    const uint8_t *base = static_cast<const uint8_t *>(blob);
-    uint64_t off[128] = {0};
-    for (uint32_t i = 0; i < h->n_sections; i++) if (sd[i].id < 128) off[sd[i].id] = sd[i].offset;
-    const uint32_t *meta = reinterpret_cast<const uint32_t *>(base + off[CB_SEC_META]);
-    cb::TableLayout lay;
-    memset(&lay, 0, sizeof(lay));
-    for (int i = 0; i < 32; i++) lay.off[i] = (uint32_t)off[i];
-    lay.uses_runtime = meta[CB_META_USES_RUNTIME];
-    lay.nV = meta[CB_META_N_VERSIONS]; lay.nRP = meta[CB_META_N_RESPATS]; lay.nS = meta[CB_META_N_SCOPES]; lay.nP = meta[CB_META_N_PRINCIPALS];
-    lay.nR = meta[CB_META_N_ROLES]; lay.nAP = meta[CB_META_N_APATS]; lay.nT = meta[CB_META_N_STRINGS]; lay.n_slots = meta[CB_META_N_SLOTS];
-    lay.n_rows = meta[CB_META_N_ROWS] ? meta[CB_META_N_ROWS] : 1;
-    lay.has_role_policies = meta[CB_META_HAS_ROLE_POLICIES]; lay.has_parent_roles = meta[CB_META_HAS_PARENT_ROLES];
-    lay.has_principal_policies = meta[CB_META_HAS_PRINCIPAL_POLICIES];
+    Setup s;
+    if (!setup(s, blob, blob_len, cols, col_bytes, n, max_actions, now, flags)) return -1;
+    cb::BatchView &b = s.b;
+    const cb::TableLayout &lay = s.lay;
     cb::TableView t;
-    t.base = base; t.L = &lay;
-
-    cb::BatchView b;
-    b.hdr0 = static_cast<const cb_hdr0 *>(cols[0]); b.hdr1 = static_cast<const cb_hdr1 *>(cols[1]);
-    b.roles = static_cast<const uint32_t *>(cols[2]); b.slots = static_cast<const uint64_t *>(cols[3]);
-    b.heap = static_cast<const uint64_t *>(cols[4]); b.bstr_off = static_cast<const uint32_t *>(cols[5]);
-    b.bstr_bytes = static_cast<const uint8_t *>(cols[6]); b.class_off = static_cast<const uint32_t *>(cols[7]);
-    b.class_pats = static_cast<const uint32_t *>(cols[8]); b.aset_k = static_cast<const uint32_t *>(cols[9]);
-    b.aset_spread = static_cast<const uint64_t *>(cols[10]);
-    b.row_am = static_cast<const uint64_t *>(cols[11]);
-    b.n_rows = meta[CB_META_N_ROWS] ? meta[CB_META_N_ROWS] : 1;
-    b.stride = n; b.first = 0; b.count = n;
-    b.role_cols = (uint32_t)(col_bytes[2] / (4 * n)); b.n_asets = (uint32_t)(col_bytes[9] / 4);
-    uint32_t km = max_actions ? max_actions : 1;
-    b.kc = 64 / b.role_cols; if (b.kc > km) b.kc = km;
-    b.n_pass = (km + b.kc - 1) / b.kc; b.max_actions = km; b.kbytes = (km + 7) / 8; b.flags = flags; b.now = now;
-    cb::finish_batch_view(b);
-    b.n_bstr = col_bytes[5] >= 4 ? (uint32_t)(col_bytes[5] / 4 - 1) : 0;
-    b.heap_words = col_bytes[4] / 8;
+    t.base = s.base; t.L = &lay;
     uint32_t status = 0;
     hostsim_deferred = 0;
-    // mode 0: what the library would pick; 1: force the general 64-bit body; 2: general 32-bit body;
-    // 3: the lean body reading a tile of the columns staged the way the kernel's TMA copies lay it out in shared memory
-    const bool narrow = b.n_pass == 1 && (uint64_t)km * b.role_cols <= 32;
-    uint32_t rcp = 1; while (rcp < b.role_cols) rcp <<= 1;
-    const bool fast = narrow && !lay.has_principal_policies && !lay.has_role_policies && !lay.has_parent_roles &&
-                      meta[CB_META_DIRECT_KINDS] && (uint64_t)lay.nR * rcp <= 64 && b.kbytes <= 4;
+    hostsim_body = 1;
+    // mode 0: the lean body reading the columns from global memory (the library's lean kernel; it gives tables whose blocks
+    // differ in shape to the unique-condition kernel, modes 4 / 5, instead); 1: force the general 64-bit body; 2: general
+    // 32-bit body; 3: the lean body reading a tile of the columns staged the way the kernel's TMA copies lay it out in shared
+    // memory.  A mode the table or batch cannot take runs the general 64-bit body.
+    const bool lean = cbhost::lean_eligible(lay, s.meta, b);
     // modes 4 / 5: the unique-condition body (cb_uc.h image) with rows read from the image / from merged 8-byte records
-    if ((mode == 4 || mode == 5) && fast) {
-        uint32_t off32[128] = {0};
-        uint64_t len64[128] = {0};
-        if (!parse_sections(blob, blob_len, off32, len64)) return -1;
-        const cbuc::Image uc = cbuc::build(base, off32, len64, meta, lay);
+    if ((mode == 4 || mode == 5) && lean) {
+        const cbuc::Image uc = cbuc::build(s.base, lay.off, s.sec_len, s.meta, lay);
         if (!uc.ok) return -3;
-        cb::TableView ut;
-        ut.base = uc.bytes.data(); ut.L = &uc.lay;
-        std::vector<cb::U4> pk((size_t)b.n_asets * b.n_rows);
-        for (size_t j = 0; j < pk.size(); j++) {
-            const cb::U4 u = ut.urows()[j % b.n_rows];
-            pk[j] = cb::uc_row_record(u, (uint32_t)b.row_am[(j / b.n_rows) * b.n_rows + u.x], b.rcp, lay.nR);
-        }
+        if (cbhost::uc_eligible(lay, uc, b)) {
+            hostsim_body = mode;
+            cb::TableView ut;
+            ut.base = uc.bytes.data(); ut.L = &uc.lay;
+            std::vector<cb::U4> pk((size_t)b.n_asets * b.n_rows);
+            for (size_t j = 0; j < pk.size(); j++) {
+                const cb::U4 u = ut.urows()[j % b.n_rows];
+                pk[j] = cb::uc_row_record(u, (uint32_t)b.row_am[(j / b.n_rows) * b.n_rows + u.x], b.rcp, lay.nR);
+            }
 #if defined(HOSTSIM_SPEC_UC)
-        // the per-string predicate words the library's pre-pass kernel would compute (one per table / batch string)
-        std::vector<uint32_t> strpred(lay.nT + b.n_bstr + 1, 0);
-        if (HostConds::n_strpred)
-            for (uint32_t id = 0; id < lay.nT + b.n_bstr; id++) strpred[id] = HostConds().strpred(ut, b, id);
-        b.strpred = strpred.data();
+            // the per-string predicate words the library's pre-pass kernel would compute (one per table / batch string)
+            std::vector<uint32_t> strpred(lay.nT + b.n_bstr + 1, 0);
+            if (HostConds::n_strpred)
+                for (uint32_t id = 0; id < lay.nT + b.n_bstr; id++) strpred[id] = HostConds().strpred(ut, b, id);
+            b.strpred = strpred.data();
 #endif
-        for (uint64_t i = 0; i < n; i++) {
-            cb::CachedCols gc; gc.b = &b; gc.n = i;
-            bool d;
-            if (mode == 5) { cb::UcRowsPacked rows; rows.pk = pk.data(); d = cb::eval_request_uc(ut, b, gc, rows, i, bitmap, nullptr, HostConds()); }
-            else { cb::UcRowsGlobal rows; rows.urows = ut.urows(); rows.row_am = b.row_am; rows.RCP = b.rcp; rows.nR = lay.nR; d = cb::eval_request_uc(ut, b, gc, rows, i, bitmap, nullptr, HostConds()); }
-            if (d) { hostsim_deferred++; cb::eval_request_general(t.base, t.L, &b, i, bitmap, nullptr, &status); }
+            for (uint64_t i = 0; i < n; i++) {
+                cb::CachedCols gc; gc.b = &b; gc.n = i;
+                bool d;
+                if (mode == 5) { cb::UcRowsPacked rows; rows.pk = pk.data(); d = cb::eval_request_uc(ut, b, gc, rows, i, bitmap, nullptr, HostConds()); }
+                else { cb::UcRowsGlobal rows; rows.urows = ut.urows(); rows.row_am = b.row_am; rows.RCP = b.rcp; rows.nR = lay.nR; d = cb::eval_request_uc(ut, b, gc, rows, i, bitmap, nullptr, HostConds()); }
+                if (d) { hostsim_deferred++; cb::eval_request_general(t.base, t.L, &b, i, bitmap, nullptr, &status); }
+            }
+            return status ? -2 : 0;
         }
-        return status ? -2 : 0;
     }
-    if (mode == 3 && fast) {
+    if (mode == 3 && lean) {
+        hostsim_body = 3;
         std::vector<uint64_t> tile(cb::tile_cols_bytes(b.role_cols, lay.n_slots) / 8 + 2);
         uint8_t *tb = reinterpret_cast<uint8_t *>(tile.data());
         for (uint64_t t0 = 0; t0 < n; t0 += cb::CB_TILE) {
@@ -129,8 +117,10 @@ extern "C" int HOSTSIM_ENTRY(const void *blob, uint64_t blob_len, uint64_t n, ui
         }
         return status ? -2 : 0;
     }
+    const bool narrow = b.n_pass == 1 && (uint64_t)b.max_actions * b.role_cols <= 32;
+    if ((mode == 0 && lean) || (mode == 2 && narrow)) hostsim_body = mode;
     for (uint64_t i = 0; i < n; i++) {
-        if (mode == 0 && fast) {
+        if (mode == 0 && lean) {
             cb::GlobalCols gc; gc.b = &b; gc.n = i;
             if (cb::eval_request_fast(t, b, gc, i, bitmap, nullptr, HostBlocks())) cb::eval_request_general(t.base, t.L, &b, i, bitmap, nullptr, &status);
         }
@@ -166,67 +156,28 @@ extern "C" void hostsim_encoded_free(void *h) { delete static_cast<HostEncoded *
 // the decision-metadata body (cb::eval_request_meta): effects + per-action metadata words + per-request metadata
 extern "C" int hostsim_check_meta(const void *blob, uint64_t blob_len, uint64_t n, uint32_t max_actions, int64_t now, uint32_t flags,
                                   const void *const *cols, const uint64_t *col_bytes, uint8_t *effects, uint32_t *action_meta, cb_request_meta *req_meta) {
-    const cb_blob_header *h = static_cast<const cb_blob_header *>(blob);
-    if (blob_len < sizeof(*h) || h->magic != CB_MAGIC || h->version != CB_VERSION) return -1;
-    const cb_section_desc *sd = reinterpret_cast<const cb_section_desc *>(static_cast<const char *>(blob) + sizeof(cb_blob_header));
-    const uint8_t *base = static_cast<const uint8_t *>(blob);
-    uint64_t off[128] = {0};
-    for (uint32_t i = 0; i < h->n_sections; i++) if (sd[i].id < 128) off[sd[i].id] = sd[i].offset;
-    const uint32_t *meta = reinterpret_cast<const uint32_t *>(base + off[CB_SEC_META]);
-    cb::TableLayout lay;
-    memset(&lay, 0, sizeof(lay));
-    for (int i = 0; i < 32; i++) lay.off[i] = (uint32_t)off[i];
-    lay.nV = meta[CB_META_N_VERSIONS]; lay.nRP = meta[CB_META_N_RESPATS]; lay.nS = meta[CB_META_N_SCOPES]; lay.nP = meta[CB_META_N_PRINCIPALS];
-    lay.nR = meta[CB_META_N_ROLES]; lay.nAP = meta[CB_META_N_APATS]; lay.nT = meta[CB_META_N_STRINGS]; lay.n_slots = meta[CB_META_N_SLOTS];
-    lay.n_rows = meta[CB_META_N_ROWS] ? meta[CB_META_N_ROWS] : 1;
-    lay.has_role_policies = meta[CB_META_HAS_ROLE_POLICIES]; lay.has_parent_roles = meta[CB_META_HAS_PARENT_ROLES];
-    lay.has_principal_policies = meta[CB_META_HAS_PRINCIPAL_POLICIES]; lay.uses_runtime = meta[CB_META_USES_RUNTIME];
-    cb::BatchView b;
-    b.hdr0 = static_cast<const cb_hdr0 *>(cols[0]); b.hdr1 = static_cast<const cb_hdr1 *>(cols[1]);
-    b.roles = static_cast<const uint32_t *>(cols[2]); b.slots = static_cast<const uint64_t *>(cols[3]);
-    b.heap = static_cast<const uint64_t *>(cols[4]); b.bstr_off = static_cast<const uint32_t *>(cols[5]);
-    b.bstr_bytes = static_cast<const uint8_t *>(cols[6]); b.class_off = static_cast<const uint32_t *>(cols[7]);
-    b.class_pats = static_cast<const uint32_t *>(cols[8]); b.aset_k = static_cast<const uint32_t *>(cols[9]);
-    b.aset_spread = static_cast<const uint64_t *>(cols[10]); b.row_am = static_cast<const uint64_t *>(cols[11]);
-    b.n_rows = lay.n_rows; b.stride = n; b.first = 0; b.count = n;
-    b.role_cols = (uint32_t)(col_bytes[2] / (4 * n)); b.n_asets = (uint32_t)(col_bytes[9] / 4);
-    uint32_t km = max_actions ? max_actions : 1;
-    b.kc = 64 / b.role_cols; if (b.kc > km) b.kc = km;
-    b.n_pass = (km + b.kc - 1) / b.kc; b.max_actions = km; b.kbytes = (km + 7) / 8; b.flags = flags; b.now = now;
-    cb::finish_batch_view(b);
-    b.n_bstr = col_bytes[5] >= 4 ? (uint32_t)(col_bytes[5] / 4 - 1) : 0;
-    b.heap_words = col_bytes[4] / 8;
+    Setup s;
+    if (!setup(s, blob, blob_len, cols, col_bytes, n, max_actions, now, flags)) return -1;
     uint32_t status = 0;
-    for (uint64_t i = 0; i < n; i++) cb::eval_request_meta(base, &lay, &b, i, effects, action_meta, req_meta, &status);
+    for (uint64_t i = 0; i < n; i++) cb::eval_request_meta(s.base, &s.lay, &s.b, i, effects, action_meta, req_meta, &status);
     return status ? -2 : 0;
 }
 // the unique-condition form of the specialised source (cb::SpecConds); "" if the table does not qualify; *n_uconds_out = distinct conditions
 extern "C" int64_t hostsim_generate_uc(const void *blob, uint64_t blob_len, char *out, uint64_t cap, uint32_t *n_uconds_out) {
-    uint32_t off[128] = {0};
-    uint64_t len[128] = {0};
-    if (!parse_sections(blob, blob_len, off, len)) return -1;
-    const uint8_t *base = static_cast<const uint8_t *>(blob);
-    const uint32_t *meta = reinterpret_cast<const uint32_t *>(base + off[CB_SEC_META]);
-    cb::TableLayout lay;
-    memset(&lay, 0, sizeof(lay));
-    for (int i = 0; i < 32; i++) lay.off[i] = off[i];
-    lay.nR = meta[CB_META_N_ROLES]; lay.n_slots = meta[CB_META_N_SLOTS];
-    const cbuc::Image uc = cbuc::build(base, off, len, meta, lay);
+    Setup s;
+    if (!setup(s, blob, blob_len)) return -1;
+    const cbuc::Image uc = cbuc::build(s.base, s.lay.off, s.sec_len, s.meta, s.lay);
     if (n_uconds_out) *n_uconds_out = uc.ok ? uc.n_uconds : 0;
-    std::string src = uc.ok ? cbspec::generate_uc(uc.bytes.data(), uc.lay.off, uc.lay.uc_conds_off, uc.n_uconds, lay.n_slots, meta[CB_META_N_CONSTS]).src : std::string();
+    std::string src = uc.ok ? cbspec::generate_uc(uc.bytes.data(), uc.lay.off, uc.lay.uc_conds_off, uc.n_uconds, s.lay.n_slots, s.meta[CB_META_N_CONSTS]).src : std::string();
     if (src.size() + 1 > cap) return -(int64_t)src.size() - 2;
     memcpy(out, src.c_str(), src.size() + 1);
     return (int64_t)src.size();
 }
 // the table-specialised block evaluators the library would hand to NVRTC (source text; "" if the table does not qualify)
 extern "C" int64_t hostsim_generate(const void *blob, uint64_t blob_len, char *out, uint64_t cap) {
-    const cb_blob_header *h = static_cast<const cb_blob_header *>(blob);
-    if (blob_len < sizeof(*h) || h->magic != CB_MAGIC || h->version != CB_VERSION) return -1;
-    const cb_section_desc *sd = reinterpret_cast<const cb_section_desc *>(static_cast<const char *>(blob) + sizeof(cb_blob_header));
-    uint32_t off[128] = {0};
-    for (uint32_t i = 0; i < h->n_sections; i++) if (sd[i].id < 128) off[sd[i].id] = (uint32_t)sd[i].offset;
-    const uint8_t *base = static_cast<const uint8_t *>(blob);
-    std::string src = cbspec::generate(base, off, reinterpret_cast<const uint32_t *>(base + off[CB_SEC_META]));
+    Setup s;
+    if (!setup(s, blob, blob_len)) return -1;
+    std::string src = cbspec::generate(s.base, s.lay.off, s.meta);
     if (src.size() + 1 > cap) return -(int64_t)src.size() - 2;
     memcpy(out, src.c_str(), src.size() + 1);
     return (int64_t)src.size();

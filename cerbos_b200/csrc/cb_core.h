@@ -84,7 +84,7 @@ struct TableView {
     CB_HD const uint32_t *dr_entries() const { return sec<uint32_t>(CB_SEC_DR_ENTRIES); }   // 4 words each
     CB_HD const uint32_t *dr_parents() const { return sec<uint32_t>(CB_SEC_DR_PARENTS); }
     CB_HD const uint32_t *dr_name_str() const { return sec<uint32_t>(CB_SEC_DR_NAME_STR); }
-    CB_HD const cb_cond *uconds() const { return reinterpret_cast<const cb_cond *>(base + L->uc_conds_off); }     // [n_uconds + 1], entry 0 unused
+    CB_HD const cb_cond *uconds() const { return reinterpret_cast<const cb_cond *>(base + L->uc_conds_off); }     // [n_uconds + 1]; entry 0: {rows of the longest scope, 0, 0, 0} (cb_uc.h)
     CB_HD const U4 *urows() const { return reinterpret_cast<const U4 *>(base + L->uc_rows_off); }                 // [n_rows] 16-byte rows, DENY first per block
     CB_HD const U4 *uc_chain() const { return reinterpret_cast<const U4 *>(base + L->uc_chain_off); }             // like RES_BLOCK_MAP: one scope-walk step each
 };
@@ -4577,10 +4577,11 @@ CB_HD bool eval_request_fast(const TableView t, const BatchView &b, const Cols &
 //   {original row index (for the batch's row x action-set masks), role8 | effect << 8, need_lo, need_hi}
 // need = bit of the rule condition | bit of the derived-role condition | bit 0: the row is satisfied iff
 // (condition word & need) == need.  What the walk consumes is the record merged with the batch:
-//   {action mask of the request's action set, need_lo, need_hi, shift of the row's role field in the role table}
+//   {action mask of the request's action set, need_lo, need_hi, shift of the row's role field in the role table | DENY << 31}
+// (the role shift stays below 64: cbhost::uc_eligible)
 CB_HD U4 uc_row_record(const U4 ur, uint32_t am, uint32_t RCP, uint32_t nR) {
-    const uint32_t role = ur.y & 0xFFu;
-    U4 r; r.x = am; r.y = ur.z; r.z = ur.w; r.w = (role == 0xFFu ? nR : role) * RCP;   // field nR of the role table = "any role"
+    const uint32_t role = ur.y & 0xFFu, deny = ((ur.y >> 8) & 0xFFu) == CB_EFFECT_DENY;
+    U4 r; r.x = am; r.y = ur.z; r.z = ur.w; r.w = (role == 0xFFu ? nR : role) * RCP | deny << 31;   // field nR of the role table = "any role"
     return r;
 }
 struct UcRowsGlobal {   // straight from the table image and the batch's row_am column
@@ -4625,6 +4626,7 @@ struct CondWord { uint64_t lo, hi; };
 enum { CB_UC_FORM_MASK32 = 0, CB_UC_FORM_MASK64 = 1, CB_UC_FORM_INDEX = 2 };
 struct GenericConds {
     static constexpr int kForm = CB_UC_FORM_MASK64;   // the condition word may use all 64 bits
+    static constexpr uint32_t kScopeRows = 0;          // rows per scope not known: the walk loops over them
     template <typename Cols>
     CB_HD Cols load(const TableView, const BatchView &, const Cols &cols) const { return cols; }
     template <typename Cols>
@@ -4652,33 +4654,54 @@ CB_HD uint32_t uc_row_pairs(const U4 r, const RP rp, const CondWord v, const uin
     const uint32_t miss = kForm == CB_UC_FORM_MASK32   ? r.y & ~vlo
                           : kForm == CB_UC_FORM_MASK64 ? (r.y & ~vlo) | (r.z & ~vhi)
                                                        : (cond_bit(v, r.y & 0xFFu) & cond_bit(v, (r.y >> 8) & 0xFFu)) ^ 1u;
-    const uint32_t rc = miss ? 0u : (uint32_t)(rp >> r.w) & role_all;
+    const uint32_t rc = miss ? 0u : (uint32_t)(rp >> (r.w & (sizeof(RP) * 8 - 1))) & role_all;
     return r.x * rc;
 }
-// The scope-chain walk of the unique-condition body: per scope the DENY rows, then the ALLOW rows, each row three or
-// four ALU operations on registers.  One 16-byte step record per scope (cb_uc.h: the chain descriptors, indexed like
-// RES_BLOCK_MAP) gives the row ranges and the next scope of the chain, so a scope costs one table load ahead of its rows.
-// RP: the role table word (32 bits when every role field fits, else 64); kForm: how the rows name their conditions
-// (known when the kernel is generated for a table).
-template <typename RP, int kForm, typename Rows>
+// Rows of one scope up to which a table-specialised walk is fully unrolled (SpecConds::kScopeRows)
+constexpr uint32_t kUcUnrollRows = 16;
+// The scope-chain walk of the unique-condition body: the rows of a scope in one pass, each row a few ALU operations on
+// registers and routed by its effect bit into the scope's DENY or ALLOW mask; since DENY beats ALLOW within a scope,
+// the DENY mask is applied first.  One pass instead of a DENY and an ALLOW loop: a warp whose lanes hit blocks of
+// different shapes pays the longest block of its lanes, not the most DENY rows plus the most ALLOW rows.  One 16-byte
+// step record per scope (cb_uc.h: the chain descriptors, indexed like RES_BLOCK_MAP) gives the row range and the next
+// scope of the chain, so a scope costs one table load ahead of its rows.
+// kRows: the longest row range of any scope of the table (0: not known); up to kUcUnrollRows the row loop is fully
+// unrolled, with no loop counter and no branch per row.  RP: the role table word (32 bits when every role field fits, else 64);
+// kForm: how the rows name their conditions (both known when the kernel is generated for a table).
+template <uint32_t kRows, typename RP, int kForm, typename Rows>
 CB_HD uint32_t uc_walk(const TableView t, const Rows rows, const RP rp, const CondWord val, const uint32_t r0, const uint32_t bm_base,
                        const uint32_t aset_base, const uint32_t role_all, uint32_t alive) {
     uint32_t allow_pairs = 0;
     const U4 *chain = t.uc_chain() + bm_base;
     for (uint32_t s = r0; s != CB_NONE32 && alive;) {
-        const U4 d = ld16(chain + s);   // {first DENY row, first ALLOW row, end of the ALLOW rows, next scope}
+        const U4 d = ld16(chain + s);   // {first row (DENY rows first), first ALLOW row, end of the rows that count, next scope}
         uint32_t D = 0, A = 0;          // DENY / ALLOW pair masks of this scope
-        uint32_t ri = d.x;
+        auto row = [&](uint32_t ri) {
+            const U4 r = rows.get(aset_base, ri);
+            const uint32_t p = uc_row_pairs<RP, kForm>(r, rp, val, role_all), deny = (uint32_t)((int32_t)r.w >> 31);
+            D |= p & deny;
+            A |= p & ~deny;
+        };
+        if constexpr (kRows != 0 && kRows <= kUcUnrollRows) {
+            // kRows rows, straight-line: an index past the end of this scope repeats its last row, which ORs in nothing
+            // new, so no row needs a branch of its own
+            if (d.x < d.z) {
+                const uint32_t last = d.z - d.x - 1;
 #if defined(__CUDA_ARCH__)
-#pragma unroll 1
+#pragma unroll
 #endif
-        for (; ri < d.y; ri++) D |= uc_row_pairs<RP, kForm>(rows.get(aset_base, ri), rp, val, role_all) & alive;
-        alive &= ~D;
+                for (uint32_t j = 0; j < kRows; j++) row(d.x + (j < last ? j : last));
+            }
+        } else {
 #if defined(__CUDA_ARCH__)
 #pragma unroll 4
 #endif
-        for (; ri < d.z; ri++) A |= uc_row_pairs<RP, kForm>(rows.get(aset_base, ri), rp, val, role_all) & alive;
-        allow_pairs |= A;   // ALLOW rows are listed only where they count (SCOPE_PERM)
+            for (uint32_t ri = d.x; ri < d.z; ri++) row(ri);
+        }
+        D &= alive;
+        alive &= ~D;
+        A &= alive;         // ALLOW rows are listed only where they count (SCOPE_PERM)
+        allow_pairs |= A;
         alive &= ~A;
         s = d.w;
     }
@@ -4725,8 +4748,9 @@ CB_HD bool eval_request_uc(const TableView t, const BatchView &b, const Cols &co
         (void)rows;
 #else
         // the role table gets one more field, "any role"; when it all fits 32 bits the per-row shift is a single SHF
-        if ((t.L->nR + 1) * RCP <= 32) allow_pairs = uc_walk<uint32_t, Conds::kForm>(t, rows, (uint32_t)rp | role_all << (t.L->nR * RCP), val, r0, bm_base, aset_base, role_all, alive0);
-        else allow_pairs = uc_walk<uint64_t, Conds::kForm>(t, rows, rp | (uint64_t)role_all << (t.L->nR * RCP), val, r0, bm_base, aset_base, role_all, alive0);
+        if ((t.L->nR + 1) * RCP <= 32)
+            allow_pairs = uc_walk<Conds::kScopeRows, uint32_t, Conds::kForm>(t, rows, (uint32_t)rp | role_all << (t.L->nR * RCP), val, r0, bm_base, aset_base, role_all, alive0);
+        else allow_pairs = uc_walk<Conds::kScopeRows, uint64_t, Conds::kForm>(t, rows, rp | (uint64_t)role_all << (t.L->nR * RCP), val, r0, bm_base, aset_base, role_all, alive0);
 #endif
         // fold: an action is ALLOWed iff some role column allowed it; then pack the stride-RC bits
         uint32_t x = allow_pairs;

@@ -34,6 +34,7 @@ struct Image {
     uint32_t n_uconds = 0, n_flat = 0;  // distinct conditions; how many of them have a flat (DNF) form
     // programs among the conditions, or rows in index form: only the run-time specialised kernel can evaluate the image
     bool needs_spec() const { return n_flat != n_uconds || n_uconds > kMaxMaskUconds; }
+    uint32_t scope_rows = 0;            // the longest row range of any chain descriptor (rows the walk visits in one scope)
     uint32_t n_gids = 0, n_gids_flat = 0;   // table conditions (per-block lists), and how many of them have a flat form
     std::vector<uint32_t> ucond_of_gid; // table condition id -> distinct condition number (1..U)
 };
@@ -53,7 +54,7 @@ inline Image build(const uint8_t *image, const uint32_t *off, const uint64_t *le
     }
     // distinct conditions
     std::map<std::tuple<uint32_t, uint32_t, uint32_t>, uint32_t> ids;
-    std::vector<uint32_t> ucond_rec;   // 4 words per distinct condition, entry 0 unused
+    std::vector<uint32_t> ucond_rec;   // 4 words per distinct condition; entry 0: {rows of the longest scope, 0, 0, 0}
     ucond_rec.assign(4, 0);
     out.ucond_of_gid.assign(n_conds, 0);
     for (uint32_t g = 0; g < n_conds; g++) {
@@ -138,9 +139,11 @@ inline Image build(const uint8_t *image, const uint32_t *off, const uint64_t *le
             d[0] = bl[0];
             d[1] = bl[0] + bl[2];
             d[2] = allow_counts ? bl[0] + bl[1] : d[1];
+            out.scope_rows = d[2] - d[0] > out.scope_rows ? d[2] - d[0] : out.scope_rows;
         }
         d[3] = next[s];
     }
+    ucond_rec[0] = out.scope_rows;   // read by cb_specialize.h: generate_uc (the unroll bound of cb::uc_walk)
     // compact image: the sections the unique-condition kernels (and the interpreter they may call) read
     out.lay = lay;
     for (auto &o : out.lay.off) o = 0;

@@ -4,7 +4,7 @@
 Generates the workload table's run-time specialised translation unit and compiles it with NVRTC exactly as a table
 load does (capi.compile_check), then prints for cb_spec_uc / cb_spec_uc_global: registers and stack, the SASS
 instruction count, the part of it inlined from cb::eval_request_uc (the per-request path), the generic byte loads
-(LD.E.U8) and the instruction count per source function (the innermost function of each instruction's line info,
+(LD.E.U8), the local-memory loads and stores (LDL / STL) and the instruction count per source function (the innermost function of each instruction's line info,
 nvdisasm -gi).  Needs the built library and the CUDA toolkit's cuobjdump / nvdisasm.
 
     python tools/uc_sass.py C3                    # the build as it is
@@ -54,7 +54,7 @@ def analyse(sass, fname, kernel):
     end = sass.find("\n.text.", start + 1)
     body = sass[start:end if end > 0 else len(sass)].splitlines()
     per_fn = collections.Counter()
-    total = req = u8 = 0
+    total = req = u8 = ldl = stl = 0
     chain, fresh = [], False
     for text in body:
         m = _LINE.search(text)
@@ -74,11 +74,13 @@ def analyse(sass, fname, kernel):
             continue
         total += 1
         u8 += op.startswith("LD.E.U8")
+        ldl += op.startswith("LDL")
+        stl += op.startswith("STL")
         fns = [fname[n] if n < len(fname) else None for n in chain]
         if "eval_request_uc" in fns:
             req += 1
         per_fn[fns[0] if fns else None] += 1
-    return {"total": total, "request_path": req, "ld_e_u8": u8, "per_fn": per_fn}
+    return {"total": total, "request_path": req, "ld_e_u8": u8, "ldl": ldl, "stl": stl, "per_fn": per_fn}
 
 
 def main():
@@ -111,7 +113,7 @@ def main():
         if r is None:
             print(f"{k}: not in this unit")
             continue
-        print(f"{k}: {usage.get(k, '?')}  instructions {r['total']}  per-request path (eval_request_uc) {r['request_path']}  LD.E.U8 {r['ld_e_u8']}")
+        print(f"{k}: {usage.get(k, '?')}  instructions {r['total']}  per-request path (eval_request_uc) {r['request_path']}  LD.E.U8 {r['ld_e_u8']}  LDL {r['ldl']}  STL {r['stl']}")
         for fn, c in r["per_fn"].most_common(a.top):
             print(f"    {c:6d}  {fn}")
 

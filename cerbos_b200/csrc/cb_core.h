@@ -3688,10 +3688,10 @@ CB_HD uint64_t uc_term_operand(const TableView t, const BatchView &b, const Cols
 // that scalar equality is plain 64-bit equality (-0.0 -> +0.0; padding = a sentinel that equals nothing) -- and every
 // membership / set predicate over it is a fully unrolled run of compares.  Lists the cache cannot hold exactly (longer,
 // container / int / NaN elements) raise `slow`: the request goes to the general body.
-// The element loops stop at `bound`: the longest list among the lanes of the warp (the device build; the host build
-// uses the list's own length), clamped to CB_LC.  It is warp-uniform, so every `if (j < bound)` below is a uniform
-// branch over a constant index (the arrays stay in registers), and positions at or above every lane's length hold only
-// padding: skipping them changes no result.
+// The element loads stop at `bound`: the longest list among the lanes of the warp (the device build; the host build
+// uses the list's own length), clamped to CB_LC.  It is warp-uniform, and positions at or above every lane's length
+// hold only padding.  The compares (list_probe) visit all CB_LC positions over constant indices (the arrays stay in
+// registers): padding equals no key, so the positions past the bound change no result.
 enum { CB_LC = 8 };
 CB_HD uint32_t list_bound(uint32_t own) {
 #if defined(__CUDA_ARCH__)
@@ -3706,7 +3706,7 @@ CB_HD uint32_t list_bound(uint32_t own) {
 // container) makes the list one "this cache cannot hold": the general body decides.
 struct ListRegs {
     uint32_t st, len;        // st 0: cached list; 1: slot ABSENT / ERROR; 2: a list this cache cannot hold exactly; 3: another type
-    uint32_t bound;          // element positions the loops visit (see above)
+    uint32_t bound;          // element positions the loads visit (see above)
     uint32_t e[CB_LC];
 };
 static constexpr uint32_t kListPad = 0xFFFFFFFEu;      // never a string id
@@ -3718,7 +3718,7 @@ static constexpr uint64_t kListBeyondHeap = 0ull;      // a word past the end of
 #else
 struct ListRegs {
     uint32_t st, len;        // st 0: cached list; 1: slot ABSENT / ERROR; 2: a list this cache cannot hold exactly; 3: another type
-    uint32_t bound;          // element positions the loops visit (see above)
+    uint32_t bound;          // element positions the loads visit (see above)
     uint64_t e[CB_LC];
 };
 static constexpr uint64_t kListPad = 0xFFFE000000000001ull;    // box tag 14: never produced by an encoder
@@ -3747,25 +3747,20 @@ CB_HD ListRegs list_load(const TableView t, const BatchView &b, uint64_t x) {
         room = (in_batch ? b.heap_words : (uint64_t)t.L->theap_words) - off;
         L.len = (uint32_t)ldg(p);
     }
-    // every element word below the bound is requested at once (bounded by the end of the heap, not by this lane's
-    // length); words beyond the length are discarded below
     L.bound = list_bound(L.len < CB_LC ? L.len : CB_LC);
-    uint64_t w[CB_LC];
-#if defined(__CUDA_ARCH__)
-#pragma unroll
-#endif
-    for (int j = 0; j < CB_LC; j++) {
-        w[j] = kListBeyondHeap;
-        if ((uint32_t)j < L.bound && (uint64_t)(j + 1) < room) w[j] = ldg(p + 1 + j);
-    }
+    // every element word below `lim` is requested at once: the warp's bound, cut at the end of the heap (element j is
+    // word j + 1 of the list).  Words past this lane's length are discarded; a word of its own that lies past the heap's
+    // end reads as kListBeyondHeap, which makes the list defer.
+    const uint32_t lim = room > (uint64_t)L.bound ? L.bound : room != 0 ? (uint32_t)room - 1u : 0u;
     bool odd = L.len > CB_LC;
 #if defined(__CUDA_ARCH__)
 #pragma unroll
 #endif
     for (int j = 0; j < CB_LC; j++) {
+        const uint64_t w = (uint32_t)j < lim ? ldg(p + 1 + j) : kListBeyondHeap;
         const bool in = (uint32_t)j < L.len;
-        odd |= in && list_elem_odd(w[j]);
-        L.e[j] = in ? list_key(w[j]) : kListPad;
+        odd |= in && list_elem_odd(w);
+        L.e[j] = in ? list_key(w) : kListPad;
     }
     if (L.st == 0) L.st = odd ? 2u : 0u;
     return L;
@@ -3785,44 +3780,66 @@ CB_HD uint64_t list_elem(const TableView t, const BatchView &b, uint64_t x, cons
     return L.e[i];   // -0.0 held as +0.0: equal under every compare a term makes
 #endif
 }
-// x in L: the outcome of in_tri() / the IN branch of term_tri() for every input this form decides, `slow` otherwise
-CB_HD int list_in_tri(uint64_t x, const ListRegs &L, bool &slow) {
-#ifdef CB_UC_STUB_LISTS
-    return (uint32_t)x == L.e[0] ? TRI_T : TRI_F;
-#endif
-    if (v64_bad(x) || L.st == 1) return TRI_E;
-    if (L.st != 0 || v64_tag(x) > CB_V64_STRING || x == CB_V64_CANON_NAN) { slow = true; return TRI_E; }
+// ---- probes: every scalar a table tests for membership in one list, compared in one pass over the list ----------------
+// The specialised evaluator (cb_specialize.h: generate_uc) turns each such scalar into a key once, compares all of a
+// list's keys in one pass right after the loads, and keeps only the hit bits: the element registers are then free for
+// the scalar terms.  A key equals an element only when the scalar is that element (padding is no key), so the status
+// logic of list_in_tri() decides whether the hit bit is the answer.
 #ifndef CB_LIST_KEYS64
-    const uint32_t nx = (uint32_t)(x >> 48) == kStringTop ? (uint32_t)x : kListNoKey;   // number / bool / null: in no list of strings
+typedef uint32_t ListKey;
+CB_HD ListKey list_probe_key(uint64_t x) { return (uint32_t)(x >> 48) == kStringTop ? (uint32_t)x : kListNoKey; }   // number / bool / null: in no list of strings
 #else
-    const uint64_t nx = norm_scalar(x);
+typedef uint64_t ListKey;
+CB_HD ListKey list_probe_key(uint64_t x) { return norm_scalar(x); }
 #endif
-    bool found = false;
+// bit p: key p equals one of L's elements.  Every key meets all CB_LC positions in straight-line code: the compares of
+// one key accumulate in a predicate, one instruction each.  Positions past the warp's bound hold padding, which no key
+// equals, so they need no bound test; dispatching on the bound instead (a branch per position, or a switch entered at
+// the bound) splits the compares into blocks across which the hit flags live in registers, and costs about three
+// instructions per compare.
+template <int P>
+CB_HD uint32_t list_probe(const ListRegs &L, const ListKey (&k)[P]) {
+    static_assert(P >= 1 && P <= 32, "one bit per key");
+#if defined(CB_UC_STUB_LISTS) || defined(CB_UC_STUB_LIST_PROBES)   // tools/uc_variants.sh: no compares (wrong results)
+    return ((uint32_t)(L.e[0] ^ k[0]) ^ L.len) & (uint32_t)((1ull << P) - 1u);
+#endif
+    uint32_t h = 0;
 #if defined(__CUDA_ARCH__)
 #pragma unroll
 #endif
-    for (int j = 0; j < CB_LC; j++)
-        if ((uint32_t)j < L.bound) found |= nx == L.e[j];
-    return found ? TRI_T : TRI_F;
-}
-// Which elements of A occur in B: bit i for element i (i < A.len).  Every set predicate over the same two list slots
-// reads this one mask (cb_specialize.h: generate_uc): one compare grid per pair instead of one per predicate.
-CB_HD uint32_t list_mask(const ListRegs &A, const ListRegs &B) {
-    uint32_t m = 0;
-#if defined(__CUDA_ARCH__)
-#pragma unroll
-#endif
-    for (int i = 0; i < CB_LC; i++) {
-        if ((uint32_t)i >= A.bound) continue;
+    for (int p = 0; p < P; p++) {
         bool hit = false;
 #if defined(__CUDA_ARCH__)
 #pragma unroll
 #endif
-        for (int j = 0; j < CB_LC; j++)
-            if ((uint32_t)j < B.bound) hit |= A.e[i] == B.e[j];
-        m |= (uint32_t)(hit && (uint32_t)i < A.len) << i;   // padding of A would "hit" the padding of B
+        for (int j = 0; j < CB_LC; j++) hit |= k[p] == L.e[j];
+        h |= (uint32_t)hit << p;
     }
-    return m;
+    return h;
+}
+// x in a list of status `st`, given hit = "x's key is one of its elements" (list_probe): the outcome of in_tri() / the
+// IN branch of term_tri() for every input this form decides, `slow` otherwise
+CB_HD int list_in_tri(uint64_t x, uint32_t st, uint32_t hit, bool &slow) {
+#ifdef CB_UC_STUB_LISTS
+    return hit ? TRI_T : TRI_F;
+#endif
+    if (v64_bad(x) || st == 1) return TRI_E;
+    if (st != 0 || v64_tag(x) > CB_V64_STRING || x == CB_V64_CANON_NAN) { slow = true; return TRI_E; }
+    return hit ? TRI_T : TRI_F;
+}
+// x in L with a probe of its own
+CB_HD int list_in_tri(uint64_t x, const ListRegs &L, bool &slow) {
+#ifdef CB_UC_STUB_LISTS
+    return (uint32_t)x == L.e[0] ? TRI_T : TRI_F;
+#endif
+    const ListKey k[1] = {list_probe_key(x)};
+    return list_in_tri(x, L.st, list_probe(L, k), slow);
+}
+// Which elements of A occur in B: bit i for element i (i < A.len), A's elements being B's probes.  Every set predicate
+// over the same two list slots reads this one mask (cb_specialize.h: generate_uc).
+CB_HD uint32_t list_mask(const ListRegs &A, const ListRegs &B) {
+    // padding of A would "hit" the padding of B; a list longer than CB_LC defers (st 2) whatever its mask
+    return list_probe(B, A.e) & (A.len < CB_LC ? (1u << A.len) - 1u : (1u << CB_LC) - 1u);
 }
 // the INTERSECTS / SUBSET branch of term_tri() from m = list_mask(A, B): isSubset(A, B) is "every element of A hit",
 // hasIntersection(A, B) -- and hasIntersection(B, A), the status tests being symmetric -- is "some element hit"

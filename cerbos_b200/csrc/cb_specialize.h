@@ -546,6 +546,29 @@ inline UcSource generate_uc(const uint8_t *uc_image, const uint32_t *off, uint32
         if (kind == CB_OPK_SLOT_ELEM && slot_list[v] && aux < 8) return "list_elem(t, b, " + sl(v) + ", " + l + ", " + std::to_string(aux) + "u)";   // CB_LC
         return "";
     };
+    // Membership terms probe their list: each list's distinct scalars (constants, slots, list[i] operands) become keys
+    // compared in one pass over the list's elements (cb_core.h: list_probe), right after the loads; the term then reads
+    // its hit bit.  At most 32 probes per list (one bit each): further terms probe on their own.
+    auto probe_operand = [&](uint32_t q) -> std::string {
+        const uint32_t *w = terms[q].data();
+        const uint32_t op = w[0] & 0xFF, xk = (w[0] >> 16) & 0xFF;
+        if (op == CB_TERM_IN_CS) return hex64(consts[w[1]]);
+        if (op == CB_TERM_IN_SS) return sl(w[1]);
+        const std::string x = operand(xk, w[1], w[3] & 0xFFFFu);
+        return !x.empty() ? x : "uc_term_operand(t, b, cols, pid, " + hex(xk) + ", " + hex(w[1]) + ", " + hex(w[3] & 0xFFFFu) + ")";
+    };
+    std::map<uint32_t, std::vector<std::string>> probes;   // list slot -> probe operands (64-bit values)
+    std::vector<uint32_t> probe_of(terms.size(), CB_NONE32);
+    for (uint32_t q = 0; q < terms.size(); q++) {
+        const uint32_t op = terms[q][0] & 0xFF;
+        if (form[q] != 'L' || (op != CB_TERM_IN_CS && op != CB_TERM_IN_SS && op != CB_TERM_IN)) continue;
+        std::vector<std::string> &ps = probes[terms[q][2]];
+        const std::string x = probe_operand(q);
+        uint32_t p = 0;
+        while (p < ps.size() && ps[p] != x) p++;
+        if (p == ps.size() && p < 32) ps.push_back(x);
+        if (p < ps.size()) probe_of[q] = p;
+    }
     auto term_code = [&](uint32_t q) -> std::string {
         const uint32_t *w = terms[q].data();
         const uint32_t op = w[0] & 0xFF, flags = (w[0] >> 8) & 0xFF, xk = (w[0] >> 16) & 0xFF, yk = w[0] >> 24;
@@ -553,11 +576,12 @@ inline UcSource generate_uc(const uint8_t *uc_image, const uint32_t *off, uint32
         const std::string x = kinds ? operand(xk, w[1], w[3] & 0xFFFFu) : "", y = kinds && op != CB_TERM_HAS ? operand(yk, w[2], w[3] >> 16) : "";
         if (form[q] == 'P') return "strpred_tri(b, " + sl(w[1]) + ", " + std::to_string(pred_of[q]) + "u)";
         if (form[q] == 'L') {
-            if (op == CB_TERM_IN_CS) return "list_in_tri(" + hex64(consts[w[1]]) + ", cols.l" + std::to_string(w[2]) + ", slow)";
-            if (op == CB_TERM_IN_SS) return "list_in_tri(" + sl(w[1]) + ", cols.l" + std::to_string(w[2]) + ", slow)";
-            if (op == CB_TERM_IN)
-                return "list_in_tri(" + (!x.empty() ? x : "uc_term_operand(t, b, cols, pid, " + hex(xk) + ", " + hex(w[1]) + ", " + hex(w[3] & 0xFFFFu) + ")") +
-                       ", cols.l" + std::to_string(w[2]) + ", slow)";
+            if (op == CB_TERM_IN_CS || op == CB_TERM_IN_SS || op == CB_TERM_IN) {
+                const std::string v = std::to_string(w[2]);
+                if (probe_of[q] == CB_NONE32) return "list_in_tri(" + probe_operand(q) + ", cols.l" + v + ", slow)";
+                const std::string xp = "x" + v + "_" + std::to_string(probe_of[q]);
+                return "list_in_tri(" + xp + ", cols.l" + v + ".st, h" + v + " & " + hex(1u << probe_of[q]) + ", slow)";
+            }
             const std::string a = std::to_string(mask_of[q].first), bb = std::to_string(mask_of[q].second);
             return std::string("list_set_tri(") + (op == CB_TERM_SUBSET ? "true" : "false") + ", cols.l" + a + ", cols.l" + bb + ", m" + a + "_" + bb + ", slow)";
         }
@@ -626,12 +650,25 @@ inline UcSource generate_uc(const uint8_t *uc_image, const uint32_t *off, uint32
     }
     s += "        (void)slow; (void)pid;\n        return bits;\n    }\n";
     s += "    CB_HD CondWord operator()(const TableView t, const BatchView &b, const SpecRegs &cols, uint32_t pid, uint64_t n, bool &slow) const {\n";
+    // the list terms first: after them only the lists' st / len and the elements that list[i] operands read stay live
+    for (const auto &pl : probes) {
+        const std::string v = std::to_string(pl.first);
+        std::string keys;
+        for (uint32_t p = 0; p < pl.second.size(); p++) {
+            const std::string xp = "x" + v + "_" + std::to_string(p);
+            s += "        const uint64_t " + xp + " = " + pl.second[p] + ";\n";
+            keys += (p ? ", list_probe_key(" : "list_probe_key(") + xp + ")";
+        }
+        s += "        const ListKey k" + v + "[" + std::to_string(pl.second.size()) + "] = {" + keys + "};\n";
+        s += "        const uint32_t h" + v + " = list_probe(cols.l" + v + ", k" + v + ");   // bit p: x" + v + "_p is an element of slot " + v + "\n";
+    }
     for (const auto &m : masks) {
         const std::string a = std::to_string(m.first.first), bb = std::to_string(m.first.second);
         s += "        const uint32_t m" + a + "_" + bb + " = list_mask(cols.l" + a + ", cols.l" + bb + ");   // elements of slot " + a + " in slot " + bb + "\n";
     }
-    for (uint32_t q = 0; q < terms.size(); q++)
-        s += "        const int q" + std::to_string(q) + " = " + term_code(q) + ";\n";
+    for (int list_terms = 1; list_terms >= 0; list_terms--)
+        for (uint32_t q = 0; q < terms.size(); q++)
+            if ((form[q] == 'L') == (list_terms == 1)) s += "        const int q" + std::to_string(q) + " = " + term_code(q) + ";\n";
     if (have_atoms) {
         s += "        Ctx c; c.t = &t; c.b = &b; c.req = n; c.pid = pid; c.unsupported = 0; c.edr = 0; c.scr_used = 0;\n";
         for (uint32_t a = 0; a < atoms.src.size(); a++) {

@@ -16,6 +16,7 @@ OK, ERR_INVALID, ERR_CUDA, ERR_UNSUPPORTED, ERR_NO_DEVICE = 0, -1, -2, -3, -4
 
 EXPORTS = [
     "cgpu_init", "cgpu_shutdown", "cgpu_table_load", "cgpu_table_retain", "cgpu_table_release", "cgpu_check", "cgpu_check_meta", "cgpu_check_narrow",
+    "cgpu_check_narrow_meta",
     "cgpu_check_device", "cgpu_sync", "cgpu_launch_count", "cgpu_deferred_count", "cgpu_table_info", "cgpu_last_kernel_config",
     "cgpu_last_cluster_config", "cgpu_profile", "cgpu_table_wait_ready", "cgpu_table_compile_check", "cgpu_peer_alloc", "cgpu_peer_open", "cgpu_peer_close",
     "cgpu_peer_free", "cgpu_peer_read", "cgpu_check_device_gather", "cgpu_gather_wait", "cgpu_last_error",
@@ -77,6 +78,9 @@ def lib():
         L.cgpu_check_narrow.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(_Batch), ctypes.POINTER(_Narrow), ctypes.c_void_p]
         L.cgpu_check_meta.restype = ctypes.c_int
         L.cgpu_check_meta.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(_Batch), ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
+        L.cgpu_check_narrow_meta.restype = ctypes.c_int
+        L.cgpu_check_narrow_meta.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(_Batch), ctypes.POINTER(_Narrow), ctypes.c_void_p,
+                                             ctypes.c_void_p, ctypes.c_void_p]
         L.cgpu_check_device.restype = ctypes.c_int
         L.cgpu_check_device.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(_Batch), ctypes.c_void_p,
                                         ctypes.c_void_p]
@@ -397,6 +401,27 @@ class Table:
         _check(lib().cgpu_check_meta(self.ctx._h, self._h, ctypes.byref(b), eff.ctypes.data_as(ctypes.c_void_p),
                                      am.ctypes.data_as(ctypes.c_void_p), rm.ctypes.data_as(ctypes.c_void_p)))
         return eff, am, rm
+
+    def check_narrow_meta(self, nb, now_ns: int = 0, flags: int = 0):
+        """cgpu_check_narrow_meta: check_meta's three outputs from a batch in the narrow wire form -- a
+        cerbos_b200.narrow.NarrowBatch, or a NarrowedBatch from the native encoder (EncodedBatch.narrow(form), whose own batch
+        flags apply; `flags` is then ignored)."""
+        from .meta import REQUEST_META_DTYPE
+        if isinstance(nb, NarrowedBatch):
+            b, nr = nb.view(now_ns)
+        else:
+            b, nr, _keep = self.prepare_narrow(nb, now_ns, flags)
+        n, km = b.n_requests, max(b.max_actions, 1)
+        eff = np.empty((n, km), dtype=np.uint8)
+        am = np.empty((n, km), dtype=np.uint32)
+        rm = np.empty(n, dtype=REQUEST_META_DTYPE)
+        self.check_narrow_meta_into(b, nr, eff.ctypes.data, am.ctypes.data, rm.ctypes.data)
+        return eff, am, rm
+
+    def check_narrow_meta_into(self, b, nr, eff_ptr, action_meta_ptr, request_meta_ptr):
+        """Zero-overhead variant for timing loops: argument blocks from prepare_narrow / NarrowedBatch.view, raw output pointers."""
+        _check(lib().cgpu_check_narrow_meta(self.ctx._h, self._h, ctypes.byref(b), ctypes.byref(nr), ctypes.c_void_p(eff_ptr),
+                                            ctypes.c_void_p(action_meta_ptr), ctypes.c_void_p(request_meta_ptr)))
 
     def check_into(self, ptrs, sizes, n, max_actions, out_ptr, now_ns=0, flags=0):
         """Zero-overhead variant for timing loops: raw host pointers in, effects written to out_ptr."""

@@ -392,7 +392,6 @@ template <class T> struct LaneBuf {
 struct cgpu_ctx {
     int device = 0;
     int sm_count = 0;
-    cudaStream_t stream = nullptr;
     uint32_t *d_status = nullptr;       // for cgpu_check_device / cgpu_sync
     std::atomic<uint64_t> launches{0};
     std::mutex mu;
@@ -426,7 +425,6 @@ struct cgpu_ctx {
     struct SliceUse { const void *ptr; cudaEvent_t done; uint8_t *stage; size_t stage_bytes; };   // stage: where the kernels write (plain device memory)
     std::vector<SliceUse> slice_uses;   // own slices whose last push to the peers may still be in flight
     std::mutex copy_mu;
-    std::mutex meta_mu;      // cgpu_check_meta calls share ctx->stream
     std::vector<cgpu_ctx *> peers;   // cgpu_init with n_devices > 1: the contexts of devices 1..n-1 (owned)
     int uc_mode = -1;        // CERBOS_B200_UC: 0 never use the unique-condition kernels, 1 whenever the table allows, unset = tables with > 1 block shape
     bool profiling = false;  // cgpu_profile(): CUDA events around the check kernel of every launch
@@ -1035,12 +1033,10 @@ int cgpu_init(const int *device_ids, int n_devices, cgpu_ctx **out) {
         cudaDeviceProp prop;
         cudaError_t ie = cudaSetDevice(ctx->device);
         if (ie == cudaSuccess) ie = cudaGetDeviceProperties(&prop, ctx->device);
-        if (ie == cudaSuccess) { ctx->sm_count = prop.multiProcessorCount; ie = cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking); }
-        if (ie == cudaSuccess) ie = cudaMalloc(&ctx->d_status, sizeof(uint32_t));
+        if (ie == cudaSuccess) { ctx->sm_count = prop.multiProcessorCount; ie = cudaMalloc(&ctx->d_status, sizeof(uint32_t)); }
         if (ie == cudaSuccess) ie = cudaMemset(ctx->d_status, 0, sizeof(uint32_t));
         if (ie != cudaSuccess) {   // nothing leaks on a failed init
             if (ctx->d_status) cudaFree(ctx->d_status);
-            if (ctx->stream) cudaStreamDestroy(ctx->stream);
             delete ctx;
             return fail(CGPU_ERR_CUDA, "cgpu_init: %s", cudaGetErrorString(ie));
         }
@@ -1091,7 +1087,6 @@ void cgpu_shutdown(cgpu_ctx *ctx) {
     if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
     for (auto e : ctx->copy_ev) if (e) cudaEventDestroy(e);
     for (auto &u : ctx->slice_uses) { if (u.done) cudaEventDestroy(u.done); if (u.stage) cudaFree(u.stage); }
-    if (ctx->stream) cudaStreamDestroy(ctx->stream);
     if (ctx->ev0) cudaEventDestroy(ctx->ev0);
     if (ctx->ev1) cudaEventDestroy(ctx->ev1);
     delete ctx;
@@ -1616,64 +1611,19 @@ void cgpu_narrowed_free(cgpu_narrowed *r) {
     delete r;
 }
 
-int cgpu_check_meta(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch, uint8_t *effects_out, uint32_t *action_meta_out, void *request_meta_out_v) {
-    cb_request_meta *request_meta_out = static_cast<cb_request_meta *>(request_meta_out_v);
-    if (!ctx || !t || !batch || !effects_out || !action_meta_out || !request_meta_out) return fail(CGPU_ERR_INVALID, "cgpu_check_meta: null argument");
-    if (t->ctx != ctx) return fail(CGPU_ERR_INVALID, "table belongs to another context");
-    const uint64_t N = batch->n_requests;
-    const uint32_t km = batch->max_actions ? batch->max_actions : 1;
-    if (N == 0) return CGPU_OK;
-    cb::BatchView hv;
-    int rc = invalid(cbhost::make_batch_view(t->desc.lay, batch, 0, N, &hv));
-    if (rc != CGPU_OK) return rc;
-    CUDA_TRY(cudaSetDevice(ctx->device));
-    // the metadata plane is the cold path (IncludeMeta requests, audit): plain stream-ordered scratch, one launch
-    cudaStream_t s = ctx->stream;
-    std::lock_guard<std::mutex> lk(ctx->meta_mu);
-    size_t offs[CGPU_N_COLUMNS + 3], total = 0;
-    for (int i = 0; i < CGPU_N_COLUMNS; i++) { offs[i] = total; total += (batch->column_bytes[i] + 255) & ~(size_t)255; }
-    offs[CGPU_N_COLUMNS] = total; total += ((size_t)N * km + 255) & ~(size_t)255;
-    offs[CGPU_N_COLUMNS + 1] = total; total += ((size_t)N * km * 4 + 255) & ~(size_t)255;
-    offs[CGPU_N_COLUMNS + 2] = total; total += ((size_t)N * sizeof(cb_request_meta) + 255) & ~(size_t)255;
-    uint8_t *dbase = nullptr;
-    CUDA_TRY(cudaMallocAsync(reinterpret_cast<void **>(&dbase), total + 4, s));
-    struct Free { uint8_t *p; cudaStream_t s; ~Free() { cudaFreeAsync(p, s); cudaStreamSynchronize(s); } } fr{dbase, s};
-    const void *dcols[CGPU_N_COLUMNS];
-    for (int i = 0; i < CGPU_N_COLUMNS; i++) {
-        dcols[i] = dbase + offs[i];
-        if (batch->column_bytes[i]) CUDA_TRY(cudaMemcpyAsync(dbase + offs[i], batch->columns[i], batch->column_bytes[i], cudaMemcpyHostToDevice, s));
-    }
-    uint32_t *d_status = reinterpret_cast<uint32_t *>(dbase + total);
-    CUDA_TRY(cudaMemsetAsync(d_status, 0, 4, s));
-    cgpu_batch db = *batch;
-    db.columns = dcols;
-    cb::BatchView bv;
-    rc = invalid(cbhost::make_batch_view(t->desc.lay, &db, 0, N, &bv));
-    if (rc != CGPU_OK) return rc;
-    uint8_t *d_eff = dbase + offs[CGPU_N_COLUMNS];
-    uint32_t *d_am = reinterpret_cast<uint32_t *>(dbase + offs[CGPU_N_COLUMNS + 1]);
-    cb_request_meta *d_rm = reinterpret_cast<cb_request_meta *>(dbase + offs[CGPU_N_COLUMNS + 2]);
-    TableDesc td = t->desc;
-    const uint64_t tiles = (N + kThreads - 1) / kThreads;
-    const uint32_t grid = (uint32_t)(tiles < (uint64_t)ctx->sm_count * 4 ? tiles : (uint64_t)ctx->sm_count * 4);
-    check_meta_kernel<<<grid, kThreads, 0, s>>>(td, bv, d_eff, d_am, d_rm, d_status);
-    CUDA_TRY(cudaGetLastError());
-    ctx->launches.fetch_add(1, std::memory_order_relaxed);
-    uint32_t st = 0;
-    CUDA_TRY(cudaMemcpyAsync(effects_out, d_eff, (size_t)N * km, cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaMemcpyAsync(action_meta_out, d_am, (size_t)N * km * 4, cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaMemcpyAsync(request_meta_out, d_rm, (size_t)N * sizeof(cb_request_meta), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaMemcpyAsync(&st, d_status, 4, cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaStreamSynchronize(s));
-    if (st) return fail(CGPU_ERR_UNSUPPORTED, "a request produced a run-time value the device cannot represent exactly (e.g. timestamp outside 1678..2262, string->double, a list longer than the scratch arena)");
-    return CGPU_OK;
-}
+// The decision-metadata outputs of a check (cgpu_check_meta / cgpu_check_narrow_meta), host buffers covering the whole batch.
+struct MetaOut {
+    uint32_t *action_meta;          // n_requests * max_actions words
+    cb_request_meta *request_meta;  // n_requests records
+};
 
-// requests [lo, hi) of `batch` on ctx's device: pipelined H2D / kernels / D2H (see below); effects_out covers the whole batch
+// requests [lo, hi) of `batch` on ctx's device: pipelined H2D / kernels / D2H (see below); effects_out covers the whole batch.
+// meta: also the metadata plane, from check_meta_kernel in place of the check kernels (nullptr: effects only)
 static inline uint32_t narrow_elem_bytes(uint32_t cl) {
     return cl == CGPU_SLOT_U64 ? 8u : (cl == CGPU_SLOT_U8 || cl == CGPU_SLOT_U8_NUM) ? 1u : cl == CGPU_SLOT_U16_ID ? 2u : 4u;
 }
-static int check_range(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch_in, uint64_t lo, uint64_t hi, uint8_t *effects_out, const cgpu_narrow *nb = nullptr) {
+static int check_range(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch_in, uint64_t lo, uint64_t hi, uint8_t *effects_out, const cgpu_narrow *nb,
+                       const MetaOut *meta) {
     // narrow form: the canonical sizes of the per-request columns (and of a 32-bit heap) are implied, not passed
     cgpu_batch batch_c = *batch_in;
     size_t cbytes[CGPU_N_COLUMNS];
@@ -1745,6 +1695,12 @@ static int check_range(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *bat
         }
         if (nb->heap_u32 || nb->heap_bits) n_heap32 = take(batch_in->column_bytes[CGPU_COL_HEAP]);
     }
+    // metadata plane: the action words and the request records
+    size_t off_am = 0, off_rm = 0;
+    if (meta) {
+        off_am = total; total += ((size_t)N * km * 4 + 255) & ~(size_t)255;
+        off_rm = total; total += ((size_t)N * sizeof(cb_request_meta) + 255) & ~(size_t)255;
+    }
     if (slot->dev_cap < total) {
         if (slot->dev) cudaFree(slot->dev);
         slot->dev = nullptr; slot->dev_cap = 0;
@@ -1760,6 +1716,8 @@ static int check_range(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *bat
     rc = invalid(cbhost::make_batch_view(t->desc.lay, &db, 0, N, &bv));
     if (rc != CGPU_OK) return rc;
     uint8_t *d_effects = dbase + offs[CGPU_N_COLUMNS];
+    uint32_t *d_am = reinterpret_cast<uint32_t *>(dbase + off_am);
+    cb_request_meta *d_rm = reinterpret_cast<cb_request_meta *>(dbase + off_rm);
 
     // Pipeline: the batch-level tables and the heap go first, then the per-request columns travel in chunks of
     // `chunk` requests -- while chunk k is evaluated, chunk k+1 is on its way in and the effect bytes of chunk k-1 on
@@ -1850,11 +1808,23 @@ static int check_range(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *bat
         cb::BatchView cv = bv;
         cv.first = c0; cv.count = cnt;
         // the kernel writes effect bytes directly (1 ALLOW / 2 DENY / 0 padding): no host post-pass
-        rc = launch_check(ctx, t, plan_launch(*ctx, *t, cv), cv, nullptr, d_effects, slot->d_status, slot->stream);
-        if (rc != CGPU_OK) return rc;
+        if (meta) {
+            const uint64_t tiles = (cnt + kThreads - 1) / kThreads;
+            const uint32_t grid = (uint32_t)(tiles < (uint64_t)ctx->sm_count * 4 ? tiles : (uint64_t)ctx->sm_count * 4);
+            check_meta_kernel<<<grid, kThreads, 0, slot->stream>>>(t->desc, cv, d_effects, d_am, d_rm, slot->d_status);
+            CUDA_TRY(cudaGetLastError());
+            ctx->launches.fetch_add(1, std::memory_order_relaxed);
+        } else {
+            rc = launch_check(ctx, t, plan_launch(*ctx, *t, cv), cv, nullptr, d_effects, slot->d_status, slot->stream);
+            if (rc != CGPU_OK) return rc;
+        }
         CUDA_TRY(cudaEventRecord(slot->ev[2 * k + 1], slot->stream));
         CUDA_TRY(cudaStreamWaitEvent(slot->d2h, slot->ev[2 * k + 1], 0));
         CUDA_TRY(cudaMemcpyAsync(effects_out + c0 * km, d_effects + c0 * km, cnt * km, cudaMemcpyDeviceToHost, slot->d2h));
+        if (meta) {
+            CUDA_TRY(cudaMemcpyAsync(meta->action_meta + c0 * km, d_am + c0 * km, cnt * km * 4, cudaMemcpyDeviceToHost, slot->d2h));
+            CUDA_TRY(cudaMemcpyAsync(meta->request_meta + c0, d_rm + c0, cnt * sizeof(cb_request_meta), cudaMemcpyDeviceToHost, slot->d2h));
+        }
     }
     CUDA_TRY(cudaMemcpyAsync(slot->h_status, slot->d_status, 4, cudaMemcpyDeviceToHost, slot->d2h));   // behind the last chunk's results
     CUDA_TRY(cudaStreamSynchronize(slot->d2h));
@@ -1866,25 +1836,16 @@ static int check_range(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *bat
     return CGPU_OK;
 }
 
-int cgpu_check_narrow(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch, const cgpu_narrow *narrow, uint8_t *effects_out) {
-    if (!ctx || !t || !batch || !narrow || !effects_out) return fail(CGPU_ERR_INVALID, "cgpu_check_narrow: null argument");
-    if (t->ctx != ctx) return fail(CGPU_ERR_INVALID, "table belongs to another context");
-    if (!narrow->roles || !narrow->slot_class || !narrow->slot_cols || narrow->role_cols == 0)
-        return fail(CGPU_ERR_INVALID, "cgpu_check_narrow: missing narrow column");
-    if (batch->n_requests == 0) return CGPU_OK;
-    return check_range(ctx, t, batch, 0, batch->n_requests, effects_out, narrow);
-}
-
-int cgpu_check(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch, uint8_t *effects_out) {
-    if (!ctx || !t || !batch || !effects_out) return fail(CGPU_ERR_INVALID, "cgpu_check: null argument");
-    if (t->ctx != ctx) return fail(CGPU_ERR_INVALID, "table belongs to another context");
+// Every host-buffer check (cgpu_check, cgpu_check_narrow, cgpu_check_meta, cgpu_check_narrow_meta) on the devices of ctx.
+// A context over several devices (cgpu_init with n_devices > 1): the requests are independent (engine.go:302-310), so the
+// batch is cut into one contiguous index range per device, each range travels over that device's own PCIe link and is
+// evaluated there; results land index-aligned in the outputs.  The narrow columns are addressed by absolute request index
+// with stride N like the wide ones, so a range of a narrow batch is cut the same way.  One host thread per device.
+static int check_sharded(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch, uint8_t *effects_out, const cgpu_narrow *nb, const MetaOut *meta) {
     const uint64_t N = batch->n_requests;
     if (N == 0) return CGPU_OK;
     const size_t n_dev = 1 + ctx->peers.size();
-    if (n_dev == 1 || N < 2 * 4096) return check_range(ctx, t, batch, 0, N, effects_out);
-    // a context over several devices (cgpu_init with n_devices > 1): the requests are independent (engine.go:302-310), so
-    // the batch is cut into one contiguous index range per device, each range travels over that device's own PCIe link
-    // and is evaluated there; results land index-aligned in effects_out.  One host thread per device.
+    if (n_dev == 1 || N < 2 * 4096) return check_range(ctx, t, batch, 0, N, effects_out, nb, meta);
     if (t->peer_tables.size() != ctx->peers.size()) return fail(CGPU_ERR_INVALID, "table was not loaded on every device of the context");
     std::vector<int> rcs(n_dev, CGPU_OK);
     std::vector<std::string> errs(n_dev);
@@ -1893,7 +1854,8 @@ int cgpu_check(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch, uint
     auto work = [&](size_t d) {
         const uint64_t lo = d * per < N ? d * per : N, hi = lo + per < N ? lo + per : N;
         if (lo >= hi) return;
-        rcs[d] = d == 0 ? check_range(ctx, t, batch, lo, hi, effects_out) : check_range(ctx->peers[d - 1], t->peer_tables[d - 1], batch, lo, hi, effects_out);
+        rcs[d] = d == 0 ? check_range(ctx, t, batch, lo, hi, effects_out, nb, meta)
+                        : check_range(ctx->peers[d - 1], t->peer_tables[d - 1], batch, lo, hi, effects_out, nb, meta);
         if (rcs[d] != CGPU_OK) errs[d] = g_err;
     };
     for (size_t d = 1; d < n_dev; d++) th.emplace_back(work, d);
@@ -1902,6 +1864,43 @@ int cgpu_check(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch, uint
     for (size_t d = 0; d < n_dev; d++)
         if (rcs[d] != CGPU_OK) return fail(rcs[d], "device %zu: %s", d, errs[d].c_str());
     return CGPU_OK;
+}
+
+// the argument checks of the narrow entry points
+static int narrow_args(const char *fn, cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch, const cgpu_narrow *narrow, const uint8_t *effects_out) {
+    if (!ctx || !t || !batch || !narrow || !effects_out) return fail(CGPU_ERR_INVALID, "%s: null argument", fn);
+    if (t->ctx != ctx) return fail(CGPU_ERR_INVALID, "table belongs to another context");
+    if (!narrow->roles || !narrow->slot_class || !narrow->slot_cols || narrow->role_cols == 0)
+        return fail(CGPU_ERR_INVALID, "%s: missing narrow column", fn);
+    return CGPU_OK;
+}
+
+int cgpu_check_narrow(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch, const cgpu_narrow *narrow, uint8_t *effects_out) {
+    const int rc = narrow_args("cgpu_check_narrow", ctx, t, batch, narrow, effects_out);
+    if (rc != CGPU_OK) return rc;
+    return check_sharded(ctx, t, batch, effects_out, narrow, nullptr);
+}
+
+int cgpu_check(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch, uint8_t *effects_out) {
+    if (!ctx || !t || !batch || !effects_out) return fail(CGPU_ERR_INVALID, "cgpu_check: null argument");
+    if (t->ctx != ctx) return fail(CGPU_ERR_INVALID, "table belongs to another context");
+    return check_sharded(ctx, t, batch, effects_out, nullptr, nullptr);
+}
+
+int cgpu_check_meta(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch, uint8_t *effects_out, uint32_t *action_meta_out, void *request_meta_out) {
+    if (!ctx || !t || !batch || !effects_out || !action_meta_out || !request_meta_out) return fail(CGPU_ERR_INVALID, "cgpu_check_meta: null argument");
+    if (t->ctx != ctx) return fail(CGPU_ERR_INVALID, "table belongs to another context");
+    const MetaOut meta{action_meta_out, static_cast<cb_request_meta *>(request_meta_out)};
+    return check_sharded(ctx, t, batch, effects_out, nullptr, &meta);
+}
+
+int cgpu_check_narrow_meta(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch, const cgpu_narrow *narrow, uint8_t *effects_out,
+                           uint32_t *action_meta_out, void *request_meta_out) {
+    if (!action_meta_out || !request_meta_out) return fail(CGPU_ERR_INVALID, "cgpu_check_narrow_meta: null argument");
+    const int rc = narrow_args("cgpu_check_narrow_meta", ctx, t, batch, narrow, effects_out);
+    if (rc != CGPU_OK) return rc;
+    const MetaOut meta{action_meta_out, static_cast<cb_request_meta *>(request_meta_out)};
+    return check_sharded(ctx, t, batch, effects_out, narrow, &meta);
 }
 
 }  // extern "C"

@@ -38,8 +38,9 @@ extern "C" {
 
 typedef struct cgpu_ctx cgpu_ctx;     /* devices + stream pools; create once per process.  n_devices = 1: one GPU (one process
                                        * per GPU under torchrun / MPI); n_devices > 1: one process drives several GPUs --
-                                       * cgpu_table_load places the table on every device, cgpu_check cuts a batch into one
-                                       * index range per device (each over its own PCIe link), results stay index-aligned */
+                                       * cgpu_table_load places the table on every device, every host-buffer cgpu_check* call
+                                       * cuts a batch into one index range per device (each over its own PCIe link), results
+                                       * stay index-aligned */
 typedef struct cgpu_table cgpu_table; /* immutable flattened rule table resident in HBM */
 
 enum cgpu_status {
@@ -185,6 +186,13 @@ void cgpu_narrowed_free(cgpu_narrowed *nb);
  * (cerbos_b200/meta.py; Go: namer.PolicyKeyFromFQN over the same ids).  An optional plane: cgpu_check moves no extra byte. */
 int cgpu_check_meta(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch, uint8_t *effects_out,
                     uint32_t *action_meta_out, void *request_meta_out /* cb_request_meta[n_requests] */);
+/* The same three outputs from a batch in the narrow wire form: inputs as cgpu_check_narrow, outputs as cgpu_check_meta.  The
+ * serving path of a host that writes audit entries or answers IncludeMeta requests: cgpu_encode -> cgpu_narrow_build ->
+ * cgpu_check_narrow_meta.  Both metadata calls run the pipeline of cgpu_check (chunked copies in and out overlapping the
+ * kernels, a stream slot per caller, every device of the context); the metadata kernel evaluates in the reference's
+ * loop order, one action after another, so a call takes 25-50x as long as cgpu_check_narrow (DESIGN.md section 7). */
+int cgpu_check_narrow_meta(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch, const cgpu_narrow *narrow, uint8_t *effects_out,
+                           uint32_t *action_meta_out, void *request_meta_out /* cb_request_meta[n_requests] */);
 
 /* Device-resident path: columns are device pointers on ctx's device.  dev_bitmap_out receives
  * n_requests * ceil(max_actions / 8) bytes, bit (k % 8) of byte n * ceil(K/8) + k / 8 set <=> ALLOW.

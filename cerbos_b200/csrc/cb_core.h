@@ -3861,6 +3861,51 @@ CB_HD int strpred_tri(const BatchView &b, uint64_t x, uint32_t p) {
     if (v64_tag(x) != CB_V64_STRING) return TRI_E;
     return (int)((ldg(b.strpred + (uint32_t)(x & 0xFFFFFFFFu)) >> p) & 1u);
 }
+// ---- typed slots: the plain-boolean branch of the specialised unique-condition evaluator ---------------------------------
+// When every slot a table's flat terms read has one type (cb_specialize.h: generate_uc), load() keeps each slot as that
+// type's payload and one per-request guard: the AND of the tests below.  Under the guard no term can be an error or
+// raise `slow`, so each term is a plain compare; a request that fails it runs the tri-state terms on its slot words.
+// string: exactly the boxed string tag with a zero payload high half (what a string id can hold)
+CB_HD bool typed_str(uint64_t x) { return (uint32_t)(x >> 32) == (uint32_t)(CB_V64_BOX_BASE | CB_V64_STRING) << 16; }
+// number: a double that is not NaN (NaN makes every ordering an error)
+CB_HD bool typed_num(uint64_t x) { const double d = u2d(x); return v64_tag(x) == 0 && d == d; }
+// bool: boxed false or true
+CB_HD bool typed_bool(uint64_t x) { return (x >> 1) == (uint64_t)(CB_V64_BOX_BASE | CB_V64_BOOL) << 47; }
+// list: cached (st 0: every element a string in registers) and long enough for the constant indices read from it
+CB_HD bool typed_list(const ListRegs &L, uint32_t need) {
+    bool ok = L.st == 0 && L.len >= need;
+#ifdef CB_LIST_KEYS64   // the elements are boxed scalars of any type: the typed terms compare string ids
+    for (int j = 0; j < CB_LC; j++) ok &= (uint32_t)j >= L.len || (uint32_t)(L.e[j] >> 48) == (CB_V64_BOX_BASE | CB_V64_STRING);
+#endif
+    return ok;
+}
+// the branch a request takes; CB_UC_STUB_FALLBACK (tools/uc_sass.py --defs, tools/uc_variants.sh): every lane takes the
+// typed one, so the unit holds the path a guarded request runs and nothing else (wrong results for the others)
+CB_HD bool uc_typed(bool guard) {
+#ifdef CB_UC_STUB_FALLBACK
+    return guard || true;
+#endif
+    return guard;
+}
+// the string id of a typed string slot (its probe key) or of element i of a typed list
+CB_HD uint32_t typed_id(uint64_t key) { return (uint32_t)key; }
+CB_HD uint64_t typed_box(uint32_t id) { return ((uint64_t)(CB_V64_BOX_BASE | CB_V64_STRING) << 48) | id; }
+// the orderings of ord_tri() / cmp_tri() on two numbers that are not NaN
+CB_HD bool typed_ord(uint32_t ci, double dx, double dy) { return ci == 2 ? dx < dy : ci == 3 ? dx <= dy : ci == 4 ? dx > dy : dx >= dy; }
+// predicate p of a string (strpred_tri() of a typed string)
+CB_HD bool typed_strpred(const BatchView &b, uint32_t id, uint32_t p) {
+#ifdef CB_UC_STUB_STRPRED
+    return ((id >> p) & 1u) != 0;
+#endif
+    return ((ldg(b.strpred + id) >> p) & 1u) != 0;
+}
+// list_probe_key(list_elem(x, L, i)) without the slot word x unless the registers do not hold the element (st 2)
+template <typename Cols>
+CB_HD ListKey list_elem_key(const TableView t, const BatchView &b, const Cols &cols, uint32_t v, const ListRegs &L, uint32_t i) {
+    if (L.st == 2) return list_probe_key(elem_operand(t, b, cols.slot(v), i));
+    return list_probe_key(list_elem(t, b, 0ull, L, i));
+}
+
 // a one-value column accessor: evaluates a term for a given string (the predicate pre-pass)
 struct OneCols {
     uint64_t x;

@@ -14,6 +14,7 @@
 #include <stdint.h>
 
 #include <cstdio>
+#include <cstring>
 #include <map>
 #include <string>
 #include <vector>
@@ -549,23 +550,28 @@ inline UcSource generate_uc(const uint8_t *uc_image, const uint32_t *off, uint32
     // Membership terms probe their list: each list's distinct scalars (constants, slots, list[i] operands) become keys
     // compared in one pass over the list's elements (cb_core.h: list_probe), right after the loads; the term then reads
     // its hit bit.  At most 32 probes per list (one bit each): further terms probe on their own.
-    auto probe_operand = [&](uint32_t q) -> std::string {
+    struct Probe {
+        uint32_t kind, v, aux;   // the operand (CB_OPK_*); kind CB_NONE32: one operand() has no register form for
+        std::string value;       // its 64-bit value as source text
+    };
+    auto probe_operand = [&](uint32_t q) -> Probe {
         const uint32_t *w = terms[q].data();
         const uint32_t op = w[0] & 0xFF, xk = (w[0] >> 16) & 0xFF;
-        if (op == CB_TERM_IN_CS) return hex64(consts[w[1]]);
-        if (op == CB_TERM_IN_SS) return sl(w[1]);
+        if (op == CB_TERM_IN_CS) return Probe{CB_OPK_CONST, w[1], 0, hex64(consts[w[1]])};
+        if (op == CB_TERM_IN_SS) return Probe{CB_OPK_SLOT, w[1], 0, sl(w[1])};
         const std::string x = operand(xk, w[1], w[3] & 0xFFFFu);
-        return !x.empty() ? x : "uc_term_operand(t, b, cols, pid, " + hex(xk) + ", " + hex(w[1]) + ", " + hex(w[3] & 0xFFFFu) + ")";
+        if (!x.empty()) return Probe{xk, w[1], w[3] & 0xFFFFu, x};
+        return Probe{CB_NONE32, 0, 0, "uc_term_operand(t, b, cols, pid, " + hex(xk) + ", " + hex(w[1]) + ", " + hex(w[3] & 0xFFFFu) + ")"};
     };
-    std::map<uint32_t, std::vector<std::string>> probes;   // list slot -> probe operands (64-bit values)
+    std::map<uint32_t, std::vector<Probe>> probes;   // list slot -> probe operands
     std::vector<uint32_t> probe_of(terms.size(), CB_NONE32);
     for (uint32_t q = 0; q < terms.size(); q++) {
         const uint32_t op = terms[q][0] & 0xFF;
         if (form[q] != 'L' || (op != CB_TERM_IN_CS && op != CB_TERM_IN_SS && op != CB_TERM_IN)) continue;
-        std::vector<std::string> &ps = probes[terms[q][2]];
-        const std::string x = probe_operand(q);
+        std::vector<Probe> &ps = probes[terms[q][2]];
+        const Probe x = probe_operand(q);
         uint32_t p = 0;
-        while (p < ps.size() && ps[p] != x) p++;
+        while (p < ps.size() && ps[p].value != x.value) p++;
         if (p == ps.size() && p < 32) ps.push_back(x);
         if (p < ps.size()) probe_of[q] = p;
     }
@@ -578,7 +584,7 @@ inline UcSource generate_uc(const uint8_t *uc_image, const uint32_t *off, uint32
         if (form[q] == 'L') {
             if (op == CB_TERM_IN_CS || op == CB_TERM_IN_SS || op == CB_TERM_IN) {
                 const std::string v = std::to_string(w[2]);
-                if (probe_of[q] == CB_NONE32) return "list_in_tri(" + probe_operand(q) + ", cols.l" + v + ", slow)";
+                if (probe_of[q] == CB_NONE32) return "list_in_tri(" + probe_operand(q).value + ", cols.l" + v + ", slow)";
                 const std::string xp = "x" + v + "_" + std::to_string(probe_of[q]);
                 return "list_in_tri(" + xp + ", cols.l" + v + ".st, h" + v + " & " + hex(1u << probe_of[q]) + ", slow)";
             }
@@ -607,18 +613,189 @@ inline UcSource generate_uc(const uint8_t *uc_image, const uint32_t *off, uint32
     for (uint32_t v = 0; v < ns; v++) n_reg += slot_used[v] || slot_list[v];
     if (n_reg > kMaxRegSlots)
         for (uint32_t v = 0; v < ns; v++) if (!slot_list[v]) slot_used[v] = false;
+    // Typed branch: one type per register slot, inferred from the terms that read it -- 'S' string (compared with a
+    // string, P.id or another string slot, a string predicate's operand, a probe key), 'N' number (ordered or compared
+    // with a number), 'B' bool (compared with a bool), 'L' cached list.  When every register slot has exactly one type,
+    // load() keeps the slots as typed payloads plus a per-request guard (cb_core.h: typed_*), and every term becomes a
+    // plain boolean under that guard; lanes that fail it evaluate today's tri-state terms on their reloaded slot words.
+    std::vector<char> ty(ns, 0);
+    std::vector<uint32_t> list_need(ns, 0);   // per list slot: 1 + the largest constant index read from it
+    bool typed = n_reg > 0 && n_reg <= kMaxRegSlots;
+    auto want = [&](uint32_t v, char k) {   // k = 0: an operand no typed term can take
+        if (v >= ns || !k) { typed = false; return; }
+        if (ty[v] && ty[v] != k) typed = false;
+        ty[v] = k;
+    };
+    auto const_type = [&](uint64_t c) -> char {
+        const uint32_t tag = v64_tag(c);
+        double d;
+        memcpy(&d, &c, sizeof d);
+        if (tag == 0) return d == d ? 'N' : 0;   // a NaN constant orders as an error
+        if (tag == CB_V64_STRING) return (uint32_t)(c >> 32) == (uint32_t)(CB_V64_BOX_BASE | CB_V64_STRING) << 16 ? 'S' : 0;
+        if (tag == CB_V64_BOOL) return (c >> 1) == (uint64_t)(CB_V64_BOX_BASE | CB_V64_BOOL) << 47 ? 'B' : 0;
+        return 0;
+    };
+    // the type an operand of a generic shape names (0: none a typed term can take); slots get it through want()
+    auto operand_type = [&](uint32_t kind, uint32_t v, uint32_t aux) -> char {
+        if (kind == CB_OPK_CONST) return const_type(consts[v]);
+        if (kind == CB_OPK_PID) return 'S';
+        if (v >= ns || !slot_list[v] || (kind == CB_OPK_SLOT_ELEM && aux >= 8)) return kind == CB_OPK_SLOT ? 0 : 'X';
+        if (kind == CB_OPK_SLOT_SIZE) return 'N';
+        if (kind == CB_OPK_SLOT_ELEM) { list_need[v] = aux + 1 > list_need[v] ? aux + 1 : list_need[v]; return 'S'; }
+        return 0;
+    };
+    // x in [constants]: the elements' one type (0: mixed, a NaN or a container, or more than term_expr() inlines)
+    auto in_const_type = [&](uint32_t q) -> char {
+        const uint64_t *p = theap + (consts[terms[q][2]] & 0xFFFFFFFFFFFFull);
+        if (p[0] == 0 || p[0] > 16) return 0;
+        char k = const_type(p[1]);
+        for (uint32_t j = 1; j < (uint32_t)p[0]; j++) k = const_type(p[1 + j]) == k ? k : 0;
+        return k == 'S' || k == 'N' ? k : 0;
+    };
+    for (uint32_t q = 0; q < terms.size() && typed; q++) {
+        const uint32_t *w = terms[q].data();
+        const uint32_t op = w[0] & 0xFF, xk = (w[0] >> 16) & 0xFF, yk = w[0] >> 24;
+        switch (op) {
+        case CB_TERM_EQ_SS: case CB_TERM_ORD_SS: break;   // typed by their other terms
+        case CB_TERM_EQ_SC: want(w[1], const_type(consts[w[2]])); break;
+        case CB_TERM_ORD_SC: want(w[1], const_type(consts[w[2]]) == 'N' ? 'N' : 0); break;
+        case CB_TERM_EQ_SP: want(w[1], 'S'); break;
+        case CB_TERM_IN_SC: want(w[1], in_const_type(q)); break;
+        case CB_TERM_IN_SS: want(w[1], 'S'); want(w[2], 'L'); break;
+        case CB_TERM_IN_CS: want(w[2], 'L'); break;
+        default: {
+            if (op == CB_TERM_HAS) { if (xk != CB_OPK_SLOT) typed = false; break; }
+            const char tx = operand_type(xk, w[1], w[3] & 0xFFFFu), tyy = operand_type(yk, w[2], w[3] >> 16);
+            if (tx == 'X' || tyy == 'X') { typed = false; break; }
+            if (form[q] == 'L') {
+                if (op == CB_TERM_IN) { if (xk == CB_OPK_SLOT) want(w[1], 'S'); want(w[2], 'L'); }
+                else { want(w[1], 'L'); want(w[2], 'L'); }
+                break;
+            }
+            if (op == CB_TERM_STARTS || op == CB_TERM_ENDS || op == CB_TERM_CONTAINS) {
+                if (xk == CB_OPK_SLOT) want(w[1], 'S');
+                if (yk == CB_OPK_SLOT) want(w[2], 'S');
+                break;
+            }
+            // CMP: a slot takes the type of what it is compared with
+            if (xk == CB_OPK_SLOT && yk != CB_OPK_SLOT) want(w[1], tyy);
+            if (yk == CB_OPK_SLOT && xk != CB_OPK_SLOT) want(w[2], tx);
+            break;
+        }
+        }
+    }
+    for (uint32_t v = 0; v < ns && typed; v++) {
+        if (slot_list[v]) want(v, 'L');
+        if ((slot_used[v] || slot_list[v]) && (!ty[v] || atoms.slot_used[v])) typed = false;   // untyped, or leaf programs read the word
+    }
+    // a scalar operand as source text of its payload type: string id 'S', double 'N', bool 'B' (k = 0, "": not a scalar
+    // the typed branch holds -- a list slot, a constant of another type)
+    auto typed_operand = [&](uint32_t kind, uint32_t v, uint32_t aux, char &k) -> std::string {
+        const std::string V = std::to_string(v);
+        if (kind == CB_OPK_CONST) {
+            const uint64_t c = consts[v];
+            k = const_type(c);
+            if (k == 'S') return hex((uint32_t)c);
+            if (k == 'N') return "u2d(" + hex64(c) + ")";
+            if (k == 'B') return c & 1u ? "true" : "false";
+            return "";
+        }
+        if (kind == CB_OPK_PID) { k = 'S'; return "pid"; }
+        if (kind == CB_OPK_SLOT_SIZE) { k = 'N'; return "(double)cols.l" + V + ".len"; }
+        if (kind == CB_OPK_SLOT_ELEM) { k = 'S'; return "typed_id(cols.l" + V + ".e[" + std::to_string(aux) + "])"; }
+        k = v < ns && (ty[v] == 'S' || ty[v] == 'N' || ty[v] == 'B') ? ty[v] : 0;
+        return k == 'S' ? "typed_id(cols.k" + V + ")" : k == 'N' ? "cols.d" + V : k == 'B' ? "cols.b" + V : "";
+    };
+    // per term: the plain boolean it is under the guard ("" = no typed form: the table gets no typed branch)
+    auto typed_term = [&](uint32_t q) -> std::string {
+        const uint32_t *w = terms[q].data();
+        const uint32_t op = w[0] & 0xFF, flags = (w[0] >> 8) & 0xFF, xk = (w[0] >> 16) & 0xFF, yk = w[0] >> 24, ci = flags & CB_TERM_CI_MASK;
+        if (form[q] == 'P') return "typed_strpred(b, typed_id(cols.k" + std::to_string(w[1]) + "), " + std::to_string(pred_of[q]) + "u)";
+        if (form[q] == 'L') {
+            if (op == CB_TERM_IN_CS || op == CB_TERM_IN_SS || op == CB_TERM_IN) {
+                if (probe_of[q] == CB_NONE32) return "";
+                if (op == CB_TERM_IN_CS && const_type(consts[w[1]]) == 0) return "";   // NaN / null / containers: not a plain membership
+                if (op == CB_TERM_IN && xk == CB_OPK_CONST && const_type(consts[w[1]]) == 0) return "";
+                return "(h" + std::to_string(w[2]) + " & " + hex(1u << probe_of[q]) + ") != 0u";
+            }
+            const std::string a = std::to_string(mask_of[q].first), bb = std::to_string(mask_of[q].second);
+            return op == CB_TERM_SUBSET ? "m" + a + "_" + bb + " == (1u << cols.l" + a + ".len) - 1u" : "m" + a + "_" + bb + " != 0u";
+        }
+        char kx = 0, ky = 0;
+        std::string x, y;
+        switch (op) {
+        case CB_TERM_EQ_SS: case CB_TERM_ORD_SS:
+            x = typed_operand(CB_OPK_SLOT, w[1], 0, kx); y = typed_operand(CB_OPK_SLOT, w[2], 0, ky);
+            if (!kx || kx != ky) return "";   // list == list: containers, the tri-state terms defer them
+            if (op == CB_TERM_EQ_SS) return x + " == " + y;
+            return kx == 'N' ? "typed_ord(" + hex(ci) + ", " + x + ", " + y + ")" : "";
+        case CB_TERM_EQ_SC: case CB_TERM_ORD_SC:
+            x = typed_operand(CB_OPK_SLOT, w[1], 0, kx); y = typed_operand(CB_OPK_CONST, w[2], 0, ky);
+            if (!kx || kx != ky) return "";
+            if (op == CB_TERM_EQ_SC) return x + " == " + y;
+            return kx == 'N' ? "typed_ord(" + hex(ci) + ", " + x + ", " + y + ")" : "";
+        case CB_TERM_EQ_SP: return "typed_id(cols.k" + std::to_string(w[1]) + ") == pid";
+        case CB_TERM_IN_SC: {
+            const uint64_t *p = theap + (consts[w[2]] & 0xFFFFFFFFFFFFull);
+            x = typed_operand(CB_OPK_SLOT, w[1], 0, kx);
+            if (!kx || kx != in_const_type(q)) return "";
+            std::string e;
+            for (uint32_t j = 0; j < (uint32_t)p[0]; j++)
+                e += std::string(j ? " | " : "") + "(" + x + " == " + (kx == 'S' ? hex((uint32_t)p[1 + j]) : "u2d(" + hex64(p[1 + j]) + ")") + ")";
+            return e;
+        }
+        case CB_TERM_HAS: return "true";
+        case CB_TERM_CMP:
+            x = typed_operand(xk, w[1], w[3] & 0xFFFFu, kx); y = typed_operand(yk, w[2], w[3] >> 16, ky);
+            if (!kx || !ky) return "";
+            if (ci == 0) return kx == ky ? x + " == " + y : "false";   // scalars of two types are not equal
+            return kx == 'N' && ky == 'N' ? "typed_ord(" + hex(ci) + ", " + x + ", " + y + ")" : "";
+        case CB_TERM_STARTS: case CB_TERM_ENDS: case CB_TERM_CONTAINS:
+            x = typed_operand(xk, w[1], w[3] & 0xFFFFu, kx); y = typed_operand(yk, w[2], w[3] >> 16, ky);
+            if (kx != 'S' || ky != 'S') return "";
+            return "str_tri(t, b, " + std::to_string(op) + "u, typed_box(" + x + "), typed_box(" + y + ")) == TRI_T";
+        default: return "";
+        }
+    };
+    std::vector<std::string> tterm(terms.size());
+    for (uint32_t q = 0; q < terms.size() && typed; q++) {
+        tterm[q] = typed_term(q);
+        typed = !tterm[q].empty();
+    }
+    // probe keys from the typed registers ("": none): a string slot's register is its probe key, an element of a list
+    // its key without the slot word (cb_core.h: list_elem_key), a constant's or P.id's key folds
+    auto probe_key = [&](const Probe &x) -> std::string {
+        const std::string V = std::to_string(x.v);
+        if (x.kind == CB_OPK_CONST || x.kind == CB_OPK_PID) return "list_probe_key(" + x.value + ")";
+        if (x.kind == CB_OPK_SLOT) return x.v < ns && ty[x.v] == 'S' ? "cols.k" + V : "";
+        if (x.kind == CB_OPK_SLOT_ELEM) return "list_elem_key(t, b, cols, " + V + "u, cols.l" + V + ", " + std::to_string(x.aux) + "u)";
+        return "";
+    };
+    for (const auto &pl : probes)
+        for (const Probe &x : pl.second) typed &= !probe_key(x).empty();
     std::string s;
     s += "// generated by cb_specialize.h (generate_uc) from the loaded table: every distinct condition, straight-line\n";
     s += "namespace cb {\n";
     for (const std::string &a : atoms.src) s += a;
+    auto reg = [&](uint32_t v) { return slot_used[v] || slot_list[v]; };
     s += "struct SpecRegs {\n    CachedCols g;\n";
     for (uint32_t v = 0; v < ns; v++)
-        if (slot_used[v] || slot_list[v]) s += "    uint64_t s" + std::to_string(v) + ";\n";
+        if (reg(v)) s += "    uint64_t s" + std::to_string(v) + ";\n";
+    if (typed) {
+        // the words above are read by load() alone (slot() reloads them): only the typed payloads live on
+        s += "    bool typed;   // every slot below holds the type its terms compare it as (SpecConds::load)\n";
+        for (uint32_t v = 0; v < ns; v++) {
+            const std::string V = std::to_string(v);
+            if (ty[v] == 'S') s += "    ListKey k" + V + ";   // string: its probe key (the id when typed)\n";
+            if (ty[v] == 'N') s += "    double d" + V + ";\n";
+            if (ty[v] == 'B') s += "    bool b" + V + ";\n";
+        }
+    }
     for (uint32_t v = 0; v < ns; v++)
         if (slot_list[v]) s += "    ListRegs l" + std::to_string(v) + ";\n";
     s += "    CB_HD uint64_t slot(uint32_t v) const {\n        switch (v) {\n";
-    for (uint32_t v = 0; v < ns; v++)
-        if (slot_used[v] || slot_list[v]) s += "        case " + std::to_string(v) + "u: return s" + std::to_string(v) + ";\n";
+    for (uint32_t v = 0; v < ns && !typed; v++)
+        if (reg(v)) s += "        case " + std::to_string(v) + "u: return s" + std::to_string(v) + ";\n";
     s += "        default: return v < " + std::to_string(ns) + "u ? g.slot(v) : (uint64_t)(CB_V64_BOX_BASE | CB_V64_ERROR) << 48;\n        }\n    }\n};\n";
     s += "struct SpecConds {\n    static constexpr uint32_t n_strpred = " + std::to_string(n_pred_bits) + "u;\n";
     s += std::string("    static constexpr int kForm = ") + (n_uconds <= 31 ? "CB_UC_FORM_MASK32" : n_uconds <= 63 ? "CB_UC_FORM_MASK64" : "CB_UC_FORM_INDEX") + ";   // how the rows name their conditions\n";
@@ -626,9 +803,25 @@ inline UcSource generate_uc(const uint8_t *uc_image, const uint32_t *off, uint32
     s += std::string("    static constexpr bool kPrograms = ") + (have_atoms ? "true" : "false") + ";   // leaf programs: needs the value helpers of cb_core.h\n";
     s += "    template <typename Cols>\n    CB_HD SpecRegs load(const TableView t, const BatchView &b, const Cols &c) const {\n        SpecRegs r;\n        r.g.b = c.b; r.g.n = c.n;\n";
     for (uint32_t v = 0; v < ns; v++)
-        if (slot_used[v] || slot_list[v]) s += "        r.s" + std::to_string(v) + " = c.slot(" + std::to_string(v) + "u);\n";
-    for (uint32_t v = 0; v < ns; v++)
-        if (slot_list[v]) s += "        r.l" + std::to_string(v) + " = list_load(t, b, r.s" + std::to_string(v) + ");\n";
+        if (reg(v)) s += "        r.s" + std::to_string(v) + " = c.slot(" + std::to_string(v) + "u);\n";
+    if (typed) {
+        // the slot words die here: what stays live is the typed payloads and the guard
+        std::string guard;
+        for (uint32_t v = 0; v < ns; v++) {
+            const std::string V = std::to_string(v);
+            if (!reg(v)) continue;
+            if (ty[v] == 'L') s += "        r.l" + V + " = list_load(t, b, r.s" + V + ");\n";
+            if (ty[v] == 'S') s += "        r.k" + V + " = list_probe_key(r.s" + V + ");\n";
+            if (ty[v] == 'N') s += "        r.d" + V + " = u2d(r.s" + V + ");\n";
+            if (ty[v] == 'B') s += "        r.b" + V + " = (r.s" + V + " & 1u) != 0;\n";
+            guard += std::string(guard.empty() ? "" : " & ") + (ty[v] == 'L' ? "typed_list(r.l" + V + ", " + std::to_string(list_need[v]) + "u)"
+                                                                 : std::string(ty[v] == 'S' ? "typed_str" : ty[v] == 'N' ? "typed_num" : "typed_bool") + "(r.s" + V + ")");
+        }
+        s += "        r.typed = " + guard + ";\n";
+    } else {
+        for (uint32_t v = 0; v < ns; v++)
+            if (slot_list[v]) s += "        r.l" + std::to_string(v) + " = list_load(t, b, r.s" + std::to_string(v) + ");\n";
+    }
     s += "        return r;\n    }\n";
     s += "    // the predicate word of one string (pre-pass over the string dictionary; bit p = predicate p holds)\n";
     s += "    CB_HD uint32_t strpred(const TableView t, const BatchView &b, uint32_t id) const {\n";
@@ -651,13 +844,15 @@ inline UcSource generate_uc(const uint8_t *uc_image, const uint32_t *off, uint32
     s += "        (void)slow; (void)pid;\n        return bits;\n    }\n";
     s += "    CB_HD CondWord operator()(const TableView t, const BatchView &b, const SpecRegs &cols, uint32_t pid, uint64_t n, bool &slow) const {\n";
     // the list terms first: after them only the lists' st / len and the elements that list[i] operands read stay live
+    // (typed: the keys come from the registers, the probe operands' values only in the tri-state branch)
+    const std::string in = typed ? "            " : "        ";
     for (const auto &pl : probes) {
         const std::string v = std::to_string(pl.first);
         std::string keys;
         for (uint32_t p = 0; p < pl.second.size(); p++) {
             const std::string xp = "x" + v + "_" + std::to_string(p);
-            s += "        const uint64_t " + xp + " = " + pl.second[p] + ";\n";
-            keys += (p ? ", list_probe_key(" : "list_probe_key(") + xp + ")";
+            if (!typed) s += "        const uint64_t " + xp + " = " + pl.second[p].value + ";\n";
+            keys += std::string(p ? ", " : "") + (typed ? probe_key(pl.second[p]) : "list_probe_key(" + xp + ")");
         }
         s += "        const ListKey k" + v + "[" + std::to_string(pl.second.size()) + "] = {" + keys + "};\n";
         s += "        const uint32_t h" + v + " = list_probe(cols.l" + v + ", k" + v + ");   // bit p: x" + v + "_p is an element of slot " + v + "\n";
@@ -666,41 +861,70 @@ inline UcSource generate_uc(const uint8_t *uc_image, const uint32_t *off, uint32
         const std::string a = std::to_string(m.first.first), bb = std::to_string(m.first.second);
         s += "        const uint32_t m" + a + "_" + bb + " = list_mask(cols.l" + a + ", cols.l" + bb + ");   // elements of slot " + a + " in slot " + bb + "\n";
     }
+    std::string tri;   // the tri-state terms and conditions (the whole evaluator without the typed branch)
+    if (typed)
+        for (const auto &pl : probes)
+            for (uint32_t p = 0; p < pl.second.size(); p++)
+                tri += in + "const uint64_t x" + std::to_string(pl.first) + "_" + std::to_string(p) + " = " + pl.second[p].value + ";\n";
     for (int list_terms = 1; list_terms >= 0; list_terms--)
         for (uint32_t q = 0; q < terms.size(); q++)
-            if ((form[q] == 'L') == (list_terms == 1)) s += "        const int q" + std::to_string(q) + " = " + term_code(q) + ";\n";
+            if ((form[q] == 'L') == (list_terms == 1)) tri += in + "const int q" + std::to_string(q) + " = " + term_code(q) + ";\n";
+    std::string atom_src;
     if (have_atoms) {
-        s += "        Ctx c; c.t = &t; c.b = &b; c.req = n; c.pid = pid; c.unsupported = 0; c.edr = 0; c.scr_used = 0;\n";
+        atom_src += "        Ctx c; c.t = &t; c.b = &b; c.req = n; c.pid = pid; c.unsupported = 0; c.edr = 0; c.scr_used = 0;\n";
         for (uint32_t a = 0; a < atoms.src.size(); a++) {
             const std::string A = std::to_string(a);
             if (atom_pred[a] >= 0) {
                 const std::string P = std::to_string(atom_pred[a]), V = sl(atoms.only_slot[a]);
-                s += "        bool a" + A + ";\n        {\n            const uint64_t x = " + V + ";\n            const uint32_t w = v64_tag(x) == CB_V64_STRING && !v64_bad(x) ? ldg(b.strpred + (uint32_t)(x & 0xFFFFFFFFu)) >> " + P + " : 2u;\n";
-                s += "            if (w & 2u) { c.scr_used = 0; a" + A + " = uc_atom_" + A + "(c, cols); } else a" + A + " = (w & 1u) != 0;\n        }\n";
+                atom_src += "        bool a" + A + ";\n        {\n            const uint64_t x = " + V + ";\n            const uint32_t w = v64_tag(x) == CB_V64_STRING && !v64_bad(x) ? ldg(b.strpred + (uint32_t)(x & 0xFFFFFFFFu)) >> " + P + " : 2u;\n";
+                atom_src += "            if (w & 2u) { c.scr_used = 0; a" + A + " = uc_atom_" + A + "(c, cols); } else a" + A + " = (w & 1u) != 0;\n        }\n";
             } else {
-                s += "        c.scr_used = 0; const bool a" + A + " = uc_atom_" + A + "(c, cols);\n";
+                atom_src += "        c.scr_used = 0; const bool a" + A + " = uc_atom_" + A + "(c, cols);\n";
             }
         }
-        s += "        slow |= c.unsupported != 0;   // a value the device forms cannot hold: the general kernel reports it\n";
-    } else s += "        (void)n;\n";
-    s += "        CondWord val; val.lo = 1ull; val.hi = 0ull;\n";
+        atom_src += "        slow |= c.unsupported != 0;   // a value the device forms cannot hold: the general kernel reports it\n";
+    } else atom_src += "        (void)n;\n";
+    std::string typed_src;
+    std::vector<std::string> cond_src(n_uconds + 1);   // per distinct condition: its tri-state block, or its program line
+    if (typed) {
+        typed_src += "        if (uc_typed(cols.typed)) {   // every term a plain boolean: no error, no deferral\n";
+        for (uint32_t q = 0; q < terms.size(); q++) typed_src += "            const bool t" + std::to_string(q) + " = " + tterm[q] + ";\n";
+    }
     for (uint32_t u = 1; u <= n_uconds; u++) {
         const uint32_t *cd = uconds + 4 * u;
         const std::string word = u < 64 ? "val.lo" : "val.hi", sh = std::to_string(u & 63u);
         if (!formula[u].empty()) {
-            s += "        " + word + " |= (uint64_t)(" + formula[u] + ") << " + sh + ";   // distinct condition " + std::to_string(u) + " (program)\n";
+            cond_src[u] = "        " + word + " |= (uint64_t)(" + formula[u] + ") << " + sh + ";   // distinct condition " + std::to_string(u) + " (program)\n";
             continue;
         }
         const uint32_t nt = cd[3] & 0xFFFFu, negate = (cd[3] >> 24) & 1u;
-        s += "        {   // distinct condition " + std::to_string(u) + "\n            bool any = false, group = true;\n";
+        std::string &c = cond_src[u];
+        c += in + "{   // distinct condition " + std::to_string(u) + "\n" + in + "    bool any = false, group = true;\n";
+        std::string any, group;   // typed: an OR of ANDs of literals
         for (uint32_t i = 0; i < nt; i++) {
             const uint32_t *w = code + 2 * (cd[2] + 2 * i);
             const uint32_t flags = (w[0] >> 8) & 0xFFu;
             const uint32_t q = term_ids[{w[0] & kUseMask, w[1], w[2], w[3]}];
-            s += "            group &= term_lit(q" + std::to_string(q) + ", " + hex(flags) + ");\n";
-            if (flags & CB_TERM_GROUP_END) s += "            any |= group; group = true;\n";
+            c += in + "    group &= term_lit(q" + std::to_string(q) + ", " + hex(flags) + ");\n";
+            group += std::string(group.empty() ? "" : " & ") + (flags & CB_TERM_LIT_F ? "!t" : "t") + std::to_string(q);
+            if (flags & CB_TERM_GROUP_END) {
+                c += in + "    any |= group; group = true;\n";
+                any += std::string(any.empty() ? "" : " | ") + "(" + group + ")";
+                group.clear();
+            }
         }
-        s += "            " + word + std::string(" |= (uint64_t)(any != ") + (negate ? "true" : "false") + ") << " + sh + ";\n        }\n";
+        c += in + "    " + word + std::string(" |= (uint64_t)(any != ") + (negate ? "true" : "false") + ") << " + sh + ";\n" + in + "}\n";
+        if (any.empty()) any = "false";
+        typed_src += "            " + word + " |= (uint64_t)(" + (negate ? "!(" + any + ")" : any) + ") << " + sh + ";   // condition " + std::to_string(u) + "\n";
+    }
+    if (typed) {
+        s += atom_src + "        CondWord val; val.lo = 1ull; val.hi = 0ull;\n" + typed_src + "        } else {   // the tri-state terms on the slot words, reloaded (cols.slot)\n" + tri;
+        for (uint32_t u = 1; u <= n_uconds; u++) if (formula[u].empty()) s += cond_src[u];
+        s += "        }\n";
+        for (uint32_t u = 1; u <= n_uconds; u++) if (!formula[u].empty()) s += cond_src[u];
+    } else {
+        s += tri + atom_src + "        CondWord val; val.lo = 1ull; val.hi = 0ull;\n";
+        for (uint32_t u = 1; u <= n_uconds; u++) s += cond_src[u];
     }
     s += "        return val;\n    }\n};\n}  // namespace cb\n";
     out.src = s;

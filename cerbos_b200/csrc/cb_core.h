@@ -46,6 +46,9 @@ struct TableLayout {
     uint32_t image_bytes;
     // "unique condition" image (cb_uc.h): offsets of the three derived sections, number of distinct conditions (0 = none)
     uint32_t uc_conds_off, uc_rows_off, uc_chain_off, n_uconds;
+    uint32_t uc_n_rows;                     // merged records per action set: slots (segment form), else image rows
+    uint32_t uc_slots_off;                  // segment form: the image row of every slot (CB_NONE32: unused), else 0
+    uint32_t uc_deny_rows, uc_allow_rows;   // slots of every block's DENY / ALLOW segment (0 / 0: row ranges)
     uint32_t theap_words;   // 8-byte words in THEAP
     uint32_t uses_runtime;  // a condition reads runtime.effectiveDerivedRoles
 };
@@ -86,6 +89,7 @@ struct TableView {
     CB_HD const uint32_t *dr_name_str() const { return sec<uint32_t>(CB_SEC_DR_NAME_STR); }
     CB_HD const cb_cond *uconds() const { return reinterpret_cast<const cb_cond *>(base + L->uc_conds_off); }     // [n_uconds + 1]; entry 0: {rows of the longest scope, 0, 0, 0} (cb_uc.h)
     CB_HD const U4 *urows() const { return reinterpret_cast<const U4 *>(base + L->uc_rows_off); }                 // [n_rows] 16-byte rows, DENY first per block
+    CB_HD const uint32_t *uc_slots() const { return reinterpret_cast<const uint32_t *>(base + L->uc_slots_off); }  // [uc_n_rows] segment form: image row per slot
     CB_HD const U4 *uc_chain() const { return reinterpret_cast<const U4 *>(base + L->uc_chain_off); }             // like RES_BLOCK_MAP: one scope-walk step each
 };
 
@@ -4646,13 +4650,51 @@ CB_HD U4 uc_row_record(const U4 ur, uint32_t am, uint32_t RCP, uint32_t nR) {
     U4 r; r.x = am; r.y = ur.z; r.z = ur.w; r.w = (role == 0xFFu ? nR : role) * RCP | deny << 31;   // field nR of the role table = "any role"
     return r;
 }
+// In the segment form (cb_uc.h) the walk reads slots: slot j of a segment is the merged record of the image row the slot
+// table names, without the DENY bit (the slot's position gives the effect, so the role shift needs no mask), or the zero
+// record for an unused slot (action mask 0: it contributes nothing).  The row sources below give both: get(ri), the
+// record of image row ri (row-range form), and slot(j), the record of slot j (segment form); the walk knows the form.
+// aset() binds them to a request's action set, at(first) moves slot() to a segment's first slot, so that the walk reads
+// the slots of one scope at constant offsets.
+CB_HD U4 uc_slot_record(const U4 r, bool used) {
+    U4 z; z.x = used ? r.x : 0u; z.y = r.y; z.z = r.z; z.w = r.w & 0x7FFFFFFFu;
+    return z;
+}
 struct UcRowsGlobal {   // straight from the table image and the batch's row_am column
     const U4 *urows; const uint64_t *row_am; uint32_t RCP, nR;
-    CB_HD U4 get(uint32_t aset_base, uint32_t ri) const { const U4 ur = ld16(urows + ri); return uc_row_record(ur, (uint32_t)ldg(row_am + aset_base + ur.x), RCP, nR); }
+    const uint32_t *slots = nullptr;   // the slot table (set by aset())
+    CB_HD UcRowsGlobal aset(const TableView t, const BatchView &b, uint32_t a) const {
+        UcRowsGlobal r = *this;
+        r.row_am += (uint64_t)a * b.n_rows;
+        r.slots = t.uc_slots();
+        return r;
+    }
+    CB_HD UcRowsGlobal at(uint32_t first) const { UcRowsGlobal r = *this; r.slots += first; return r; }
+    CB_HD U4 get(uint32_t ri) const { const U4 ur = ld16(urows + ri); return uc_row_record(ur, (uint32_t)ldg(row_am + ur.x), RCP, nR); }
+    CB_HD U4 slot(uint32_t j) const { const uint32_t ri = ldg(slots + j); return uc_slot_record(get(ri != CB_NONE32 ? ri : 0u), ri != CB_NONE32); }
+    // what the library's merges store at position j of an action set (cb_kernels.h: check_uc_body; uc_merge_rows)
+    CB_HD U4 merged(const TableView t, uint32_t j) const { return t.L->uc_slots_off ? slot(j) : get(j); }
 };
-struct UcRowsPacked {   // one merged record per (action set, row), built once per CTA in shared memory
+// Merged records in shared memory (or from the launch's pre-pass).  by_slot: one per (action set, slot) in the segment
+// form, as the library merges them (UcRowsGlobal::merged); else one per (action set, image row), and slot() reaches a
+// slot's record through the slot table.
+struct UcRowsPacked {
     const U4 *pk;
-    CB_HD U4 get(uint32_t aset_base, uint32_t ri) const { return ld16(pk + aset_base + ri); }
+    bool by_slot = false;
+    const uint32_t *slots = nullptr;   // records per image row: the slot table (set by aset())
+    CB_HD UcRowsPacked aset(const TableView t, const BatchView &b, uint32_t a) const {
+        UcRowsPacked r = *this;
+        r.pk = pk + a * (by_slot ? t.L->uc_n_rows : b.n_rows);
+        r.slots = t.uc_slots();
+        return r;
+    }
+    CB_HD UcRowsPacked at(uint32_t first) const { UcRowsPacked r = *this; if (by_slot) r.pk += first; else r.slots += first; return r; }
+    CB_HD U4 get(uint32_t ri) const { return ld16(pk + ri); }
+    CB_HD U4 slot(uint32_t j) const {
+        if (by_slot) return ld16(pk + j);
+        const uint32_t ri = ldg(slots + j);
+        return uc_slot_record(ld16(pk + (ri != CB_NONE32 ? ri : 0u)), ri != CB_NONE32);
+    }
 };
 
 // column access with L1 allocation: the eager condition pass reads the same slot from several terms
@@ -4686,9 +4728,13 @@ struct CachedCols {
 // kernels only): rows carry the two condition NUMBERS they need instead of a mask.
 struct CondWord { uint64_t lo, hi; };
 enum { CB_UC_FORM_MASK32 = 0, CB_UC_FORM_MASK64 = 1, CB_UC_FORM_INDEX = 2 };
+// Rows of one scope up to which a table-specialised walk is fully unrolled: the DENY + ALLOW slots of the image's segment
+// form (cb_uc.h; SpecConds::kDenyRows / kAllowRows)
+constexpr uint32_t kUcUnrollRows = 16;
+constexpr uint32_t kUcRowsOfLayout = ~0u;   // Conds::kDenyRows / kAllowRows of a build not generated for one table
 struct GenericConds {
     static constexpr int kForm = CB_UC_FORM_MASK64;   // the condition word may use all 64 bits
-    static constexpr uint32_t kScopeRows = 0;          // rows per scope not known: the walk loops over them
+    static constexpr uint32_t kDenyRows = kUcRowsOfLayout, kAllowRows = kUcRowsOfLayout;   // the image's form is read at run time
     template <typename Cols>
     CB_HD Cols load(const TableView, const BatchView &, const Cols &cols) const { return cols; }
     template <typename Cols>
@@ -4710,59 +4756,68 @@ struct GenericConds {
 
 // (action x role column) pairs of one row if its conditions hold: a needed condition bit that is clear zeroes the role columns
 CB_HD uint32_t cond_bit(const CondWord v, uint32_t u) { return (uint32_t)(((u & 64u) ? v.hi : v.lo) >> (u & 63u)) & 1u; }
+// shift: the row's role field in the role table, below the bits of RP
 template <typename RP, int kForm>
-CB_HD uint32_t uc_row_pairs(const U4 r, const RP rp, const CondWord v, const uint32_t role_all) {
+CB_HD uint32_t uc_row_pairs(const U4 r, const RP rp, const CondWord v, const uint32_t role_all, const uint32_t shift) {
     const uint32_t vlo = (uint32_t)v.lo, vhi = (uint32_t)(v.lo >> 32);
     const uint32_t miss = kForm == CB_UC_FORM_MASK32   ? r.y & ~vlo
                           : kForm == CB_UC_FORM_MASK64 ? (r.y & ~vlo) | (r.z & ~vhi)
                                                        : (cond_bit(v, r.y & 0xFFu) & cond_bit(v, (r.y >> 8) & 0xFFu)) ^ 1u;
-    const uint32_t rc = miss ? 0u : (uint32_t)(rp >> (r.w & (sizeof(RP) * 8 - 1))) & role_all;
+    const uint32_t rc = miss ? 0u : (uint32_t)(rp >> shift) & role_all;
     return r.x * rc;
 }
-// Rows of one scope up to which a table-specialised walk is fully unrolled (SpecConds::kScopeRows)
-constexpr uint32_t kUcUnrollRows = 16;
-// The scope-chain walk of the unique-condition body: the rows of a scope in one pass, each row a few ALU operations on
-// registers and routed by its effect bit into the scope's DENY or ALLOW mask; since DENY beats ALLOW within a scope,
-// the DENY mask is applied first.  One pass instead of a DENY and an ALLOW loop: a warp whose lanes hit blocks of
-// different shapes pays the longest block of its lanes, not the most DENY rows plus the most ALLOW rows.  One 16-byte
-// step record per scope (cb_uc.h: the chain descriptors, indexed like RES_BLOCK_MAP) gives the row range and the next
-// scope of the chain, so a scope costs one table load ahead of its rows.
-// kRows: the longest row range of any scope of the table (0: not known); up to kUcUnrollRows the row loop is fully
-// unrolled, with no loop counter and no branch per row.  RP: the role table word (32 bits when every role field fits, else 64);
-// kForm: how the rows name their conditions (both known when the kernel is generated for a table).
-template <uint32_t kRows, typename RP, int kForm, typename Rows>
+// The scope-chain walk of the unique-condition body.  One 16-byte step record per scope (cb_uc.h: the chain descriptors,
+// indexed like RES_BLOCK_MAP) locates the scope's rows and gives the next scope of the chain, so a scope costs one table
+// load ahead of its rows.  Each row is a few ALU operations on registers; since DENY beats ALLOW within a scope, the
+// scope's DENY mask is applied first.
+//   segment form (cb_uc.h): every scope runs the same kDenyRows DENY slots, then kAllowRows ALLOW slots, at constant
+//     offsets from its segment; unused slots are zero records.  Known when the kernel is generated for the table (up to
+//     kUcUnrollRows in all), the slots are straight-line code with no clamp, effect test or loop state per row.  Per
+//     scope, the descriptor's masks route the ALLOW slots: into the DENY mask for a block of DENY rows alone, and to
+//     nothing where the scope's ALLOWs do not count (SCOPE_PERM).
+//   row ranges (longer scopes): one loop over the scope's rows, each routed by its effect bit into the DENY or ALLOW
+//     mask, so that a warp whose lanes hit blocks of different shapes pays the longest block of its lanes, not the most
+//     DENY rows plus the most ALLOW rows.
+// kDenyRows / kAllowRows: the segment slots (both 0: row ranges; kUcRowsOfLayout: read from the layout).  RP: the role
+// table word (32 bits when every role field fits, else 64); kForm: how the rows name their conditions.
+template <uint32_t kDenyRows, uint32_t kAllowRows, typename RP, int kForm, typename Rows>
 CB_HD uint32_t uc_walk(const TableView t, const Rows rows, const RP rp, const CondWord val, const uint32_t r0, const uint32_t bm_base,
-                       const uint32_t aset_base, const uint32_t role_all, uint32_t alive) {
+                       const uint32_t role_all, uint32_t alive) {
+    constexpr bool kOfLayout = kDenyRows == kUcRowsOfLayout;
+    const uint32_t n_deny = kOfLayout ? t.L->uc_deny_rows : kDenyRows, n_allow = kOfLayout ? t.L->uc_allow_rows : kAllowRows;
+    const bool segments = n_deny + n_allow != 0;
     uint32_t allow_pairs = 0;
     const U4 *chain = t.uc_chain() + bm_base;
     for (uint32_t s = r0; s != CB_NONE32 && alive;) {
-        const U4 d = ld16(chain + s);   // {first row (DENY rows first), first ALLOW row, end of the rows that count, next scope}
+        const U4 d = ld16(chain + s);   // segments: {first slot, ALLOW mask, DENY mask of the ALLOW slots, next scope}; else {first row (DENY rows first), first ALLOW row, end of the rows that count, next scope}
         uint32_t D = 0, A = 0;          // DENY / ALLOW pair masks of this scope
-        auto row = [&](uint32_t ri) {
-            const U4 r = rows.get(aset_base, ri);
-            const uint32_t p = uc_row_pairs<RP, kForm>(r, rp, val, role_all), deny = (uint32_t)((int32_t)r.w >> 31);
-            D |= p & deny;
-            A |= p & ~deny;
-        };
-        if constexpr (kRows != 0 && kRows <= kUcUnrollRows) {
-            // kRows rows, straight-line: an index past the end of this scope repeats its last row, which ORs in nothing
-            // new, so no row needs a branch of its own
-            if (d.x < d.z) {
-                const uint32_t last = d.z - d.x - 1;
+        if (segments) {
+            const Rows seg = rows.at(d.x);
+            auto slot = [&](uint32_t j) { const U4 r = seg.slot(j); return uc_row_pairs<RP, kForm>(r, rp, val, role_all, r.w); };
 #if defined(__CUDA_ARCH__)
 #pragma unroll
 #endif
-                for (uint32_t j = 0; j < kRows; j++) row(d.x + (j < last ? j : last));
-            }
+            for (uint32_t j = 0; j < n_deny; j++) D |= slot(j);
+#if defined(__CUDA_ARCH__)
+#pragma unroll
+#endif
+            for (uint32_t j = 0; j < n_allow; j++) A |= slot(n_deny + j);
+            D |= A & d.z;   // a block of DENY rows alone fills both parts
+            A &= d.y;
         } else {
 #if defined(__CUDA_ARCH__)
 #pragma unroll 4
 #endif
-            for (uint32_t ri = d.x; ri < d.z; ri++) row(ri);
+            for (uint32_t ri = d.x; ri < d.z; ri++) {
+                const U4 r = rows.get(ri);
+                const uint32_t p = uc_row_pairs<RP, kForm>(r, rp, val, role_all, r.w & (sizeof(RP) * 8 - 1)), deny = (uint32_t)((int32_t)r.w >> 31);
+                D |= p & deny;
+                A |= p & ~deny;
+            }
         }
         D &= alive;
         alive &= ~D;
-        A &= alive;         // ALLOW rows are listed only where they count (SCOPE_PERM)
+        A &= alive;
         allow_pairs |= A;
         alive &= ~A;
         s = d.w;
@@ -4800,19 +4855,19 @@ CB_HD bool eval_request_uc(const TableView t, const BatchView &b, const Cols &co
         const CondWord val = conds(t, b, regs, pid, n, slow);   // bit u: distinct condition u holds; bit 0: "no condition"
         if (slow) return true;
         const uint32_t role_all = (1u << n_roles) - 1;
-        const uint32_t aset_base = aset * b.n_rows;
         const uint32_t amask = K * RC >= 32 ? b.stride_pattern : b.stride_pattern & ((1u << (K * RC)) - 1);   // bit kk*RC per action
         const uint32_t alive0 = amask * role_all;
         const uint32_t bm_base = (rv * t.L->nRP + kc) * t.L->nS;
         uint32_t allow_pairs;
 #ifdef CB_UC_STUB_WALK
-        allow_pairs = alive0 & ((uint32_t)val.lo ^ (uint32_t)(val.lo >> 32) ^ (uint32_t)rp ^ r0 ^ bm_base ^ aset_base);
+        allow_pairs = alive0 & ((uint32_t)val.lo ^ (uint32_t)(val.lo >> 32) ^ (uint32_t)rp ^ r0 ^ bm_base ^ aset);
         (void)rows;
 #else
+        const Rows arows = rows.aset(t, b, aset);
         // the role table gets one more field, "any role"; when it all fits 32 bits the per-row shift is a single SHF
         if ((t.L->nR + 1) * RCP <= 32)
-            allow_pairs = uc_walk<Conds::kScopeRows, uint32_t, Conds::kForm>(t, rows, (uint32_t)rp | role_all << (t.L->nR * RCP), val, r0, bm_base, aset_base, role_all, alive0);
-        else allow_pairs = uc_walk<Conds::kScopeRows, uint64_t, Conds::kForm>(t, rows, rp | (uint64_t)role_all << (t.L->nR * RCP), val, r0, bm_base, aset_base, role_all, alive0);
+            allow_pairs = uc_walk<Conds::kDenyRows, Conds::kAllowRows, uint32_t, Conds::kForm>(t, arows, (uint32_t)rp | role_all << (t.L->nR * RCP), val, r0, bm_base, role_all, alive0);
+        else allow_pairs = uc_walk<Conds::kDenyRows, Conds::kAllowRows, uint64_t, Conds::kForm>(t, arows, rp | (uint64_t)role_all << (t.L->nR * RCP), val, r0, bm_base, role_all, alive0);
 #endif
         // fold: an action is ALLOWed iff some role column allowed it; then pack the stride-RC bits
         uint32_t x = allow_pairs;

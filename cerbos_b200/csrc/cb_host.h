@@ -142,7 +142,8 @@ inline bool lean_eligible(const cb::TableLayout &lay, const uint32_t *meta, cons
 // The unique-condition body, on top of the lean body's conditions: a built image, 32-bit request indices and merged-row
 // counts, and a role word with room for the "any role" column nR.
 inline bool uc_eligible(const cb::TableLayout &lay, const cbuc::Image &uc, const cb::BatchView &bv) {
-    return uc.ok && (uint64_t)(lay.nR + 1) * bv.rcp <= 64 && bv.count < (1ull << 32) && (uint64_t)bv.n_asets * lay.n_rows < (1ull << 31);
+    return uc.ok && (uint64_t)(lay.nR + 1) * bv.rcp <= 64 && bv.count < (1ull << 32) && (uint64_t)bv.n_asets * lay.n_rows < (1ull << 31) &&
+           (uint64_t)bv.n_asets * uc.lay.uc_n_rows < (1ull << 31);
 }
 
 }  // namespace cbhost

@@ -301,7 +301,7 @@ __device__ __forceinline__ void check_tiles_body(const TableDesc &td, const cb::
 // CTA-wide barrier in the loop.  Deferred requests (an operand the 8-byte forms cannot decide, differing policy
 // versions) go to the launch's deferral list, drained by the general kernel right behind; they are first written as
 // DENY so that a lost deferral could only fail closed.
-// smem layout (kStaged): [image, 128-byte padded][merged rows: n_asets x n_rows x 16 B]
+// smem layout (kStaged): [image, 128-byte padded][merged rows: n_asets x uc_n_rows (slots or rows) x 16 B]
 template <typename Conds, typename Cols, bool kStaged>
 __device__ __forceinline__ void check_uc_body(const TableDesc &td, const cb::BatchView &bv, uint8_t *bitmap, uint8_t *effects, uint8_t *smem_image, uint64_t *mbar) {
     cb::TableView tv;
@@ -333,12 +333,9 @@ __device__ __forceinline__ void check_uc_body(const TableDesc &td, const cb::Bat
         if (threadIdx.x == 0) tma_load_image(smem_image, td, mbar);
         mbar_wait(mbar, 0);
         cb::U4 *pks = reinterpret_cast<cb::U4 *>(smem_image + ((td.lay.image_bytes + 127u) & ~127u));
-        const uint32_t n_pk = bv.n_asets * bv.n_rows;
-        const cb::U4 *ur = tv.urows();
-        for (uint32_t j = threadIdx.x; j < n_pk; j += kThreads) {
-            const cb::U4 u = ur[j % bv.n_rows];
-            pks[j] = cb::uc_row_record(u, (uint32_t)bv.row_am[(j / bv.n_rows) * bv.n_rows + u.x], bv.rcp, td.lay.nR);
-        }
+        const uint32_t n_u = td.lay.uc_n_rows, n_pk = bv.n_asets * n_u;
+        cb::UcRowsGlobal g; g.urows = tv.urows(); g.row_am = bv.row_am; g.RCP = bv.rcp; g.nR = td.lay.nR;
+        for (uint32_t j = threadIdx.x; j < n_pk; j += kThreads) pks[j] = g.aset(tv, bv, j / n_u).merged(tv, j % n_u);
         __syncthreads();
         pk = pks;
     }
@@ -359,7 +356,7 @@ __device__ __forceinline__ void check_uc_body(const TableDesc &td, const cb::Bat
             Cols gc;
             gc.b = &bv; gc.n = n;
             bool d;
-            if (kStaged || pk) { cb::UcRowsPacked rows; rows.pk = pk; d = cb::eval_request_uc(tv, bv, gc, rows, n, bitmap, effects, Conds()); }
+            if (kStaged || pk) { cb::UcRowsPacked rows; rows.pk = pk; rows.by_slot = true; d = cb::eval_request_uc(tv, bv, gc, rows, n, bitmap, effects, Conds()); }
             else { cb::UcRowsGlobal rows; rows.urows = tv.urows(); rows.row_am = bv.row_am; rows.RCP = bv.rcp; rows.nR = td.lay.nR; d = cb::eval_request_uc(tv, bv, gc, rows, n, bitmap, effects, Conds()); }
             if (d) {
                 cb::store_result(bv, gc, n, bitmap, effects, bv.max_actions, 0u);

@@ -436,7 +436,7 @@ inline std::string translate_program(const uint32_t *code_words, uint32_t code_o
 // generate_uc() emits `SpecConds`: load() pulls every attribute slot the conditions read into registers (all loads in
 // flight at once, coalesced), operator() evaluates every distinct DNF term once (shared between conditions) and
 // combines them into the request's condition word.  Rows stay data (16-byte records walked by cb::uc_walk,
-// unrolled to the table's longest scope).
+// unrolled over the image's DENY and ALLOW segment slots).
 // uc: the compact image (cb_uc.h) and its layout.  "" = does not qualify (a distinct condition without flat form ...).
 struct UcLimits {
     uint32_t max_terms = 512;   // distinct terms
@@ -454,7 +454,8 @@ inline UcSource generate_uc(const uint8_t *uc_image, const uint32_t *off, uint32
     Atoms atoms;
     std::vector<std::string> formula(n_uconds + 1);   // per distinct condition without flat form: boolean formula over atoms
     const uint32_t *uconds = reinterpret_cast<const uint32_t *>(uc_image + uc_conds_off);    // [n_uconds + 1] x {code_off, code_len, flat_off, flat_info}
-    const uint32_t scope_rows = uconds[0];   // record 0: {rows of the longest scope, 0, 0, 0} (cb_uc.h), the walk's unroll bound
+    // record 0 (cb_uc.h): {rows the walk visits per scope, DENY slots, ALLOW slots of the segment form (0 / 0: row ranges), 0}
+    const uint32_t scope_rows = uconds[0], deny_rows = uconds[1], allow_rows = uconds[2];
     const uint32_t *code = reinterpret_cast<const uint32_t *>(uc_image + off[CB_SEC_CODE]);
     const uint64_t *consts = reinterpret_cast<const uint64_t *>(uc_image + off[CB_SEC_CONSTS_V64]);
     const uint64_t *theap = reinterpret_cast<const uint64_t *>(uc_image + off[CB_SEC_THEAP]);
@@ -799,7 +800,9 @@ inline UcSource generate_uc(const uint8_t *uc_image, const uint32_t *off, uint32
     s += "        default: return v < " + std::to_string(ns) + "u ? g.slot(v) : (uint64_t)(CB_V64_BOX_BASE | CB_V64_ERROR) << 48;\n        }\n    }\n};\n";
     s += "struct SpecConds {\n    static constexpr uint32_t n_strpred = " + std::to_string(n_pred_bits) + "u;\n";
     s += std::string("    static constexpr int kForm = ") + (n_uconds <= 31 ? "CB_UC_FORM_MASK32" : n_uconds <= 63 ? "CB_UC_FORM_MASK64" : "CB_UC_FORM_INDEX") + ";   // how the rows name their conditions\n";
-    s += "    static constexpr uint32_t kScopeRows = " + std::to_string(scope_rows) + "u;   // rows of the longest scope (cb::uc_walk)\n";
+    s += "    static constexpr uint32_t kScopeRows = " + std::to_string(scope_rows) + "u;   // rows the walk visits per scope (cb::uc_walk)\n";
+    s += "    static constexpr uint32_t kDenyRows = " + std::to_string(deny_rows) + "u, kAllowRows = " + std::to_string(allow_rows) +
+         "u;   // segment slots (0 / 0: row ranges)\n";
     s += std::string("    static constexpr bool kPrograms = ") + (have_atoms ? "true" : "false") + ";   // leaf programs: needs the value helpers of cb_core.h\n";
     s += "    template <typename Cols>\n    CB_HD SpecRegs load(const TableView t, const BatchView &b, const Cols &c) const {\n        SpecRegs r;\n        r.g.b = c.b; r.g.n = c.n;\n";
     for (uint32_t v = 0; v < ns; v++)

@@ -4,7 +4,8 @@
 // keeps one compiled condition per rule (ruletable.go:105-416).  Across a policy set the same conditions recur: shared
 // derived roles, the same ownership / tenancy test on every resource kind.  This builder
 //   * numbers the DISTINCT conditions of the table 1..U (same DNF term list, or -- no flat form -- same bytecode program),
-//   * rewrites every row to {original index, role, effect, mask of the condition bits it needs} (16 bytes, DENY rows first per block),
+//   * rewrites every row to {original index, role, effect, mask of the condition bits it needs} (16 bytes, DENY rows first
+//     per block) and, where they fit, lays the rows out in fixed per-block DENY and ALLOW segments of slots,
 //   * copies only the sections the unique-condition kernels read into a compact image (C3: 49 KB blob -> ~10 KB),
 // so that a kernel can evaluate every distinct condition of a request once, with all lanes in lock step, and walk the
 // rows as mask algebra (cb::eval_request_uc).  Built once per cgpu_table_load; the Python blob format is unchanged.
@@ -34,7 +35,8 @@ struct Image {
     uint32_t n_uconds = 0, n_flat = 0;  // distinct conditions; how many of them have a flat (DNF) form
     // programs among the conditions, or rows in index form: only the run-time specialised kernel can evaluate the image
     bool needs_spec() const { return n_flat != n_uconds || n_uconds > kMaxMaskUconds; }
-    uint32_t scope_rows = 0;            // the longest row range of any chain descriptor (rows the walk visits in one scope)
+    uint32_t scope_rows = 0;            // rows the walk visits in one scope: deny_rows + allow_rows, else the longest row range
+    uint32_t deny_rows = 0, allow_rows = 0;   // slots of every block's DENY / ALLOW segment (0 / 0: row ranges, see build())
     uint32_t n_gids = 0, n_gids_flat = 0;   // table conditions (per-block lists), and how many of them have a flat form
     std::vector<uint32_t> ucond_of_gid; // table condition id -> distinct condition number (1..U)
 };
@@ -54,7 +56,7 @@ inline Image build(const uint8_t *image, const uint32_t *off, const uint64_t *le
     }
     // distinct conditions
     std::map<std::tuple<uint32_t, uint32_t, uint32_t>, uint32_t> ids;
-    std::vector<uint32_t> ucond_rec;   // 4 words per distinct condition; entry 0: {rows of the longest scope, 0, 0, 0}
+    std::vector<uint32_t> ucond_rec;   // 4 words per distinct condition; entry 0: {scope_rows, deny_rows, allow_rows, 0}
     ucond_rec.assign(4, 0);
     out.ucond_of_gid.assign(n_conds, 0);
     for (uint32_t g = 0; g < n_conds; g++) {
@@ -108,10 +110,12 @@ inline Image build(const uint8_t *image, const uint32_t *off, const uint64_t *le
     }
     // Chain descriptors: one step record per RES_BLOCK_MAP entry (version, kind pattern, scope s), so that the walk
     // (cb::uc_walk) reads one record per scope instead of the block map, the block, the scope flags and the parent chain:
-    //   {first DENY row, first ALLOW row, end of the ALLOW rows, next scope of the resource chain (chain_next; CB_NONE32)}
-    // A scope whose ALLOWs do not count (SCOPE_PERM != 1) lists no ALLOW rows: the walk applies a scope's ALLOW mask
-    // only where they count, so those rows can never change a result.  Not lenient-dependent: only the chain's first
-    // scope is (chain_start, per request).
+    //   row ranges: {first DENY row, first ALLOW row, end of the ALLOW rows, next scope of the resource chain (chain_next; CB_NONE32)}
+    //   segments:   {first slot of the block's segment, ALLOW mask of the scope (~0u or 0), ~0u: the ALLOW slots hold DENY rows, else 0,
+    //                next scope}
+    // A scope whose ALLOWs do not count (SCOPE_PERM != 1) lists no ALLOW rows, or gets ALLOW mask 0: the walk applies a
+    // scope's ALLOW mask only where they count, so those rows can never change a result.  Not lenient-dependent: only the
+    // chain's first scope is (chain_start, per request).
     const uint32_t nS = meta[CB_META_N_SCOPES];
     const uint64_t n_map = (uint64_t)meta[CB_META_N_VERSIONS] * meta[CB_META_N_RESPATS] * nS;
     if (nS == 0 || len[CB_SEC_SCOPE_PARENT] < (uint64_t)nS * 4 || len[CB_SEC_SCOPE_FLAGS] < (uint64_t)nS * 4 || len[CB_SEC_RES_BLOCK_MAP] < n_map * 4) {
@@ -128,22 +132,72 @@ inline Image build(const uint8_t *image, const uint32_t *off, const uint64_t *le
         if (x != CB_NONE32 && (x >= nS || steps > nS)) { out.why = "scope parent chain out of range"; return out; }
         next[s] = x;
     }
+    // Segment form: block b gets the fixed segment b + 1 of deny_rows DENY slots followed by allow_rows ALLOW slots, the
+    // same counts for every block; segment 0 stays empty for scopes without a block.  The slot section names the image
+    // row of every slot (the rows themselves stay as above); the library merges the rows with the batch in slot order
+    // (cb::UcRowsGlobal), where a slot's position gives its effect, so the merged record drops it, and an unused slot
+    // (CB_NONE32) becomes the zero record, whose action mask 0 contributes nothing.  The walk then runs a fixed number of rows per scope at constant
+    // offsets from the segment base, with no per-row clamp or effect test.  Only rows the walk can use take slots: those of
+    // blocks the block map names, and ALLOW rows only of blocks named from a scope whose ALLOWs count.  A block named only
+    // from scopes whose ALLOWs do not count has DENY rows alone; they fill its whole segment, and its descriptors route
+    // the ALLOW slots into the scope's DENY mask.  So the counts are: deny_rows, the most DENY rows of a block whose ALLOWs
+    // count; allow_rows, the most ALLOW rows of such a block, or more, so that every DENY-only block fits.  Tables whose
+    // segment would pass the unroll bound of the specialised walk (cb::kUcUnrollRows) keep the row ranges and their loop.
+    std::vector<uint8_t> used(n_blocks, 0);   // bit 0: named by the block map; bit 1: from a scope whose ALLOWs count
+    for (uint64_t e = 0; e < n_map; e++) {
+        const uint32_t bid = bmap[e];
+        if (bid == CB_NONE32) continue;
+        if (bid >= n_blocks) { out.why = "block map entry out of range"; return out; }
+        used[bid] |= 1 | (((sflags[e % nS] >> CB_SCOPE_PERM_SHIFT) & 3) == 1) << 1;
+    }
+    uint32_t max_deny = 0, max_allow = 0, max_deny_only = 0;
+    for (uint32_t b = 0; b < n_blocks; b++) {
+        const uint32_t *bl = ublocks.data() + 4 * (size_t)b;   // {row_start, n_rows, DENY rows, 0}
+        if (used[b] & 2) {
+            max_deny = bl[2] > max_deny ? bl[2] : max_deny;
+            max_allow = bl[1] - bl[2] > max_allow ? bl[1] - bl[2] : max_allow;
+        } else if (used[b]) max_deny_only = bl[2] > max_deny_only ? bl[2] : max_deny_only;
+    }
+    if (max_deny_only > max_deny + max_allow) max_allow = max_deny_only - max_deny;
+    const uint32_t seg = max_deny + max_allow;
+    const bool segments = seg >= 1 && seg <= cb::kUcUnrollRows && ((uint64_t)n_blocks + 1) * seg < (1ull << 31);
+    std::vector<uint32_t> slots;   // segment form: the image row of every slot, CB_NONE32 for an unused one
+    if (segments) {
+        out.deny_rows = max_deny;
+        out.allow_rows = max_allow;
+        slots.assign(((size_t)n_blocks + 1) * seg, CB_NONE32);
+        for (uint32_t b = 0; b < n_blocks; b++) {
+            const uint32_t *bl = ublocks.data() + 4 * (size_t)b;
+            const uint32_t n_use = (used[b] & 2) ? bl[1] : used[b] ? bl[2] : 0;
+            for (uint32_t r = 0; r < n_use; r++)   // DENY-only blocks: every row in order, over both parts
+                slots[(size_t)(b + 1) * seg + (r < bl[2] || !(used[b] & 2) ? r : max_deny + r - bl[2])] = bl[0] + r;
+        }
+    }
     std::vector<uint32_t> chain(4 * (size_t)n_map, 0);
     for (uint64_t e = 0; e < n_map; e++) {
         const uint32_t s = (uint32_t)(e % nS), bid = bmap[e];
         uint32_t *d = chain.data() + 4 * e;
-        if (bid != CB_NONE32) {
-            if (bid >= n_blocks) { out.why = "block map entry out of range"; return out; }
+        if (bid != CB_NONE32) {   // (below n_blocks: checked above)
             const uint32_t *bl = ublocks.data() + 4 * (size_t)bid;   // {row_start, n_rows, DENY rows, 0}
             const bool allow_counts = ((sflags[s] >> CB_SCOPE_PERM_SHIFT) & 3) == 1;
-            d[0] = bl[0];
-            d[1] = bl[0] + bl[2];
-            d[2] = allow_counts ? bl[0] + bl[1] : d[1];
-            out.scope_rows = d[2] - d[0] > out.scope_rows ? d[2] - d[0] : out.scope_rows;
+            if (segments) {
+                d[0] = (bid + 1) * seg;
+                d[1] = allow_counts ? ~0u : 0u;
+                d[2] = (used[bid] & 2) ? 0u : ~0u;
+            } else {
+                d[0] = bl[0];
+                d[1] = bl[0] + bl[2];
+                d[2] = allow_counts ? bl[0] + bl[1] : d[1];
+                out.scope_rows = d[2] - d[0] > out.scope_rows ? d[2] - d[0] : out.scope_rows;
+            }
         }
         d[3] = next[s];
     }
-    ucond_rec[0] = out.scope_rows;   // read by cb_specialize.h: generate_uc (the unroll bound of cb::uc_walk)
+    if (segments) out.scope_rows = seg;
+    // read by cb_specialize.h: generate_uc (the walk's form and its unroll bounds)
+    ucond_rec[0] = out.scope_rows;
+    ucond_rec[1] = out.deny_rows;
+    ucond_rec[2] = out.allow_rows;
     // compact image: the sections the unique-condition kernels (and the interpreter they may call) read
     out.lay = lay;
     for (auto &o : out.lay.off) o = 0;
@@ -161,7 +215,11 @@ inline Image build(const uint8_t *image, const uint32_t *off, const uint64_t *le
     out.lay.uc_conds_off = append(ucond_rec.data(), ucond_rec.size() * 4);
     out.lay.uc_rows_off = append(urows.data(), urows.size() * 4);
     out.lay.uc_chain_off = append(chain.data(), chain.size() * 4);
+    out.lay.uc_slots_off = segments ? append(slots.data(), slots.size() * 4) : 0;
     out.lay.n_uconds = out.n_uconds;
+    out.lay.uc_n_rows = segments ? (uint32_t)slots.size() : (uint32_t)(urows.size() / 4);
+    out.lay.uc_deny_rows = out.deny_rows;
+    out.lay.uc_allow_rows = out.allow_rows;
     out.lay.theap_words = (uint32_t)(len[CB_SEC_THEAP] / 8);
     out.lay.image_bytes = (uint32_t)out.bytes.size();
     out.ok = true;

@@ -195,8 +195,9 @@ __global__ void __launch_bounds__(kThreads) uc_merge_rows(const __grid_constant_
     if (j >= n_pk) return;
     cb::TableView tv;
     tv.base = td.base; tv.L = &td.lay;
-    const cb::U4 u = tv.urows()[j % bv.n_rows];
-    out[j] = cb::uc_row_record(u, (uint32_t)bv.row_am[(j / bv.n_rows) * bv.n_rows + u.x], bv.rcp, td.lay.nR);
+    const uint32_t n_u = td.lay.uc_n_rows;
+    cb::UcRowsGlobal g; g.urows = tv.urows(); g.row_am = bv.row_am; g.RCP = bv.rcp; g.nR = td.lay.nR;
+    out[j] = g.aset(tv, bv, j / n_u).merged(tv, j % n_u);
 }
 
 __global__ void gather_signal(const __grid_constant__ SignalParams p) {
@@ -608,7 +609,7 @@ void cache_write(const std::string &path, const std::vector<char> &data) {
 enum SpecForm { SPEC_NONE = 0, SPEC_SHAPES = 1, SPEC_UC = 2 };
 constexpr uint32_t kUcMaxSmem = 72 * 1024;   // compact image + merged rows: three CTAs / SM at least
 
-// Shared memory of a staged unique-condition launch: the compact image, then one 16-byte merged row per (action set, row).
+// Shared memory of a staged unique-condition launch: the compact image, then one 16-byte merged row per (action set, slot or image row).
 uint64_t uc_smem_bytes(const cbuc::Image &uc, uint64_t n_pk) { return (((uint64_t)uc.lay.image_bytes + 127) & ~127ull) + 16 * n_pk; }
 // Whether the staged unique-condition kernel fits with n_pk merged rows.  With one (the default) it is the question whether
 // the image leaves room at all, which decides whether the specialised translation unit carries the staged kernel.
@@ -815,7 +816,7 @@ LaunchPlan plan_launch(const cgpu_ctx &ctx, const cgpu_table &t, const cb::Batch
     // Unique-condition kernels: lean-eligible tables with <= 63 distinct conditions whose blocks differ in shape
     // (with one shape the per-shape specialised tile kernel is the better fit).  Index order, no clustering.
     // (an image with condition programs or index-form rows is only good for the specialised kernel: cbuc::Image::needs_spec)
-    const uint64_t n_pk = (uint64_t)bv.n_asets * lay.n_rows;   // merged rows: one per (action set, row)
+    const uint64_t n_pk = (uint64_t)bv.n_asets * t.uc.lay.uc_n_rows;   // merged rows: one per (action set, slot or image row)
     p.uc = p.lean && cbhost::uc_eligible(lay, t.uc, bv) && (uc_spec_ready || !t.uc.needs_spec()) && t.d_uc_image &&
            (ctx.uc_mode == 1 || (ctx.uc_mode != 0 && ctx.cluster_mode != 1 && t.meta[CB_META_BLOCK_SHAPES] > 1));   // CERBOS_B200_CLUSTER=1 keeps the clustered path reachable
     // Clustering pays when the policy blocks differ in shape (rows / conditions): with a single shape every lane runs
@@ -826,7 +827,7 @@ LaunchPlan plan_launch(const cgpu_ctx &ctx, const cgpu_table &t, const cb::Batch
     // 16-byte aligned and image + two tile stages fit the shared-memory budget of CB_MIN_BLOCKS resident CTAs.
     const uint32_t tile_bytes = cb::tile_cols_bytes(bv.role_cols, lay.n_slots);
     // [image][tile stage 0][tile stage 1][row_am copy][aset_k copy]
-    const uint64_t small_tabs = n_pk * 8 + (((uint64_t)bv.n_asets + 1) & ~1ull) * 4 + 16 + 2 * kThreads;   // + tile_s[2] + res_s[2][256]
+    const uint64_t small_tabs = (uint64_t)bv.n_asets * lay.n_rows * 8 + (((uint64_t)bv.n_asets + 1) & ~1ull) * 4 + 16 + 2 * kThreads;   // + tile_s[2] + res_s[2][256]
     const uint32_t tiles_smem = ((lay.image_bytes + 127u) & ~127u) + 2 * tile_bytes + (uint32_t)(small_tabs < 65536 ? small_tabs : 65536);
     auto al16 = [](const void *ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
     p.col_tiles = !p.uc && p.lean && p.stage && !p.cluster && !ctx.force_no_tiles && tiles_smem <= kMaxTilesSmem && bv.stride % 4 == 0 &&
@@ -925,7 +926,7 @@ int launch_check(cgpu_ctx *ctx, const cgpu_table *t, const LaunchPlan &plan, con
         uint32_t *cell = nullptr, *strpred = nullptr;
         cb::U4 *pk = nullptr;
         const uint32_t n_str = lay.nT + bv.n_bstr;
-        const uint64_t n_pk = (uint64_t)bv.n_asets * lay.n_rows;
+        const uint64_t n_pk = (uint64_t)bv.n_asets * t->uc.lay.uc_n_rows;
         int rc = acquire_defer(ctx, stream, bv.count, &defer, &cell, plan.strpred ? (size_t)n_str + 1 : 0, &strpred, plan.merge_rows ? (size_t)n_pk : 0, &pk);
         if (rc != CGPU_OK) return rc;
         if (plan.merge_rows) {

@@ -1,6 +1,7 @@
 // tools/uc_walk_steps.cpp -- host helper of tools/uc_walk_steps.py (built by it with g++, never shipped).
 // The rows the unique-condition walk (cb::uc_walk) visits per request and scope level, from the image's chain
-// descriptors: out[(i * levels + level) * 2 + {0, 1}] = DENY rows, ALLOW rows that count; zero past the end of the chain
+// descriptors (segment form: the used slots of the scope's segment): out[(i * levels + level) * 2 + {0, 1}] = DENY rows,
+// ALLOW rows that count; zero past the end of the chain
 // and for a request the walk does not reach.  The walk also stops once every pair of the request is decided, which
 // needs the condition word: not modelled.
 #include <cstdint>
@@ -40,9 +41,17 @@ extern "C" int64_t uc_walk_rows(const void *blob, uint64_t blob_len, uint64_t n,
         uint32_t lv = 0;
         for (uint32_t sc = cb::chain_start(ut, h0.z, CB_SCOPE_FLAG_RESOURCE, (b.flags & CB_BATCH_FLAG_LENIENT) != 0); sc != CB_NONE32 && lv < levels;
              sc = chain[sc].w, lv++) {
-            out[(i * levels + lv) * 2] = (uint16_t)(chain[sc].y - chain[sc].x);
-            out[(i * levels + lv) * 2 + 1] = (uint16_t)(chain[sc].z - chain[sc].y);
+            const cb::U4 d = chain[sc];
+            uint32_t n_deny = d.y - d.x, n_allow = d.z - d.y;
+            if (uc.deny_rows + uc.allow_rows) {   // segment form: the used slots (an unused one has no original row)
+                n_deny = n_allow = 0;
+                for (uint32_t j = 0; j < uc.deny_rows + uc.allow_rows; j++)
+                    if (ut.uc_slots()[d.x + j] != CB_NONE32) (j < uc.deny_rows || d.z ? n_deny : n_allow)++;
+                n_allow = d.y ? n_allow : 0;
+            }
+            out[(i * levels + lv) * 2] = (uint16_t)n_deny;
+            out[(i * levels + lv) * 2 + 1] = (uint16_t)n_allow;
         }
     }
-    return uc.scope_rows;
+    return uc.scope_rows;   // segment form: the slots every scope runs
 }

@@ -6,7 +6,8 @@ core, tools/uc_walk_steps.cpp), takes the rows each request visits per scope lev
 counts per warp of 32 consecutive requests, level by level:
   two loops   max over lanes of the DENY rows + max over lanes of the ALLOW rows (a DENY loop, then an ALLOW loop)
   one pass    max over lanes of DENY + ALLOW rows
-  unrolled    the table's longest scope at every level some lane reaches (the specialised walk's straight-line rows)
+  unrolled    the slots of the image's DENY + ALLOW segments (segment form; else the table's longest scope) at every level
+              some lane reaches (the specialised walk's straight-line rows)
 The walk also stops once every pair of a request is decided; that needs the condition values and is not modelled, so
 the counts are upper bounds.  No device needed.
 
@@ -46,7 +47,8 @@ def _helper():
 
 
 def walk_rows(blob, b, flags=0):
-    """-> (uint16[n, LEVELS, 2] DENY / counting ALLOW rows per request and level, the table's longest scope)"""
+    """-> (uint16[n, LEVELS, 2] DENY / counting ALLOW rows per request and level, the rows the walk visits per scope:
+    the segment slots, or the table's longest scope)"""
     cols = [np.ascontiguousarray(c) for c in b.columns]
     out = np.zeros((b.n, LEVELS, 2), dtype=np.uint16)
     rc = _helper().uc_walk_rows(ctypes.create_string_buffer(blob, len(blob)), ctypes.c_uint64(len(blob)), ctypes.c_uint64(b.n),
@@ -83,7 +85,7 @@ def main():
     steps = warp_steps(rows, scope_rows)
     reached = (rows.sum(axis=2) > 0).any(axis=0)
     n_lv = int(np.nonzero(reached)[0].max()) + 1 if reached.any() else 0
-    print(f"{a.workload}: {b.n} requests, {b.n // 32} full warps; longest scope {scope_rows} rows; chains up to {n_lv} levels")
+    print(f"{a.workload}: {b.n} requests, {b.n // 32} full warps; {scope_rows} unrolled rows per scope; chains up to {n_lv} levels")
     print("row steps per warp     " + "".join(f"  level {j}" for j in range(n_lv)) + "     total")
     for name, s in steps.items():
         print(f"  {name:<20}" + "".join(f"{s[:, j].mean():9.2f}" for j in range(n_lv)) + f"{s.sum(axis=1).mean():10.2f}")

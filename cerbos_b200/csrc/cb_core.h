@@ -4780,13 +4780,18 @@ CB_HD uint32_t uc_row_pairs(const U4 r, const RP rp, const CondWord v, const uin
 //     DENY rows plus the most ALLOW rows.
 // kDenyRows / kAllowRows: the segment slots (both 0: row ranges; kUcRowsOfLayout: read from the layout).  RP: the role
 // table word (32 bits when every role field fits, else 64); kForm: how the rows name their conditions.
-template <uint32_t kDenyRows, uint32_t kAllowRows, typename RP, int kForm, typename Rows>
+// obs(level, scope, D, A, condition word) sees, per scope of the chain (level 0 = r0), the pairs it newly DENY- and
+// ALLOW-decided: the metadata form records where each pair was decided; the default observer does nothing.
+struct UcNoObserver {
+    CB_HD void operator()(uint32_t, uint32_t, uint32_t, uint32_t, const CondWord &) const {}
+};
+template <uint32_t kDenyRows, uint32_t kAllowRows, typename RP, int kForm, typename Rows, typename Obs = UcNoObserver>
 CB_HD uint32_t uc_walk(const TableView t, const Rows rows, const RP rp, const CondWord val, const uint32_t r0, const uint32_t bm_base,
-                       const uint32_t role_all, uint32_t alive) {
+                       const uint32_t role_all, uint32_t alive, Obs &&obs = Obs()) {
     constexpr bool kOfLayout = kDenyRows == kUcRowsOfLayout;
     const uint32_t n_deny = kOfLayout ? t.L->uc_deny_rows : kDenyRows, n_allow = kOfLayout ? t.L->uc_allow_rows : kAllowRows;
     const bool segments = n_deny + n_allow != 0;
-    uint32_t allow_pairs = 0;
+    uint32_t allow_pairs = 0, level = 0;
     const U4 *chain = t.uc_chain() + bm_base;
     for (uint32_t s = r0; s != CB_NONE32 && alive;) {
         const U4 d = ld16(chain + s);   // segments: {first slot, ALLOW mask, DENY mask of the ALLOW slots, next scope}; else {first row (DENY rows first), first ALLOW row, end of the rows that count, next scope}
@@ -4820,6 +4825,7 @@ CB_HD uint32_t uc_walk(const TableView t, const Rows rows, const RP rp, const Co
         A &= alive;
         allow_pairs |= A;
         alive &= ~A;
+        obs(level++, s, D, A, val);
         s = d.w;
     }
     return allow_pairs;
@@ -4883,6 +4889,137 @@ CB_HD bool eval_request_uc(const TableView t, const BatchView &b, const Cols &co
         else for (uint32_t kk = 0; kk < K; kk++) acc |= ((x >> (kk * RC)) & 1) << kk;
     }
     store_result(b, cols, n, bitmap, effects, K, acc);
+    return false;
+}
+
+// ---- decision metadata from the unique-condition walk
+// eval_request_meta restated for the bit-parallel walk, on the tables cbuc::build_meta takes (resource policies only, so
+// the principal pass of the reference decides nothing and its words say NO_MATCH).  The walk decides each (action k x role
+// column i) pair at one scope level; the reference walks role column i for action k up to that level, role columns in
+// order, and stops at the first column that ALLOWs k.  Hence:
+//   * action word k: the lowest column whose pair was ALLOWed, else the lowest DENYed, at the scope that decided it;
+//     neither: no scope, source RESOURCE_POLICY (NO_MATCH without roles: the reference's role loop never runs);
+//   * effectiveDerivedRoles: the derived roles of the levels the reference visits, 0 .. the deepest decision level of a
+//     pair (k, i) with i at most the first ALLOWing column of k (an undecided pair: the chain's last level).  The walk
+//     itself may go deeper, for pairs the reference never walks.
+// The observer records every pair's decision level, bit-sliced (CB_MAX_CHAIN = 8 levels: three words).
+CB_HD uint32_t ctz32(uint32_t x) {   // x != 0
+#if defined(__CUDA_ARCH__)
+    return (uint32_t)__ffs((int)x) - 1;
+#else
+    return (uint32_t)__builtin_ctz(x);
+#endif
+}
+struct UcMetaObserver {
+    uint32_t deny = 0, lv0 = 0, lv1 = 0, lv2 = 0, levels = 0;   // DENY-decided pairs; bit b of each decided pair's level; levels walked
+    CB_HD void operator()(uint32_t level, uint32_t, uint32_t D, uint32_t A, const CondWord &) {
+        const uint32_t dec = D | A;
+        deny |= D;
+        lv0 |= (level & 1u) ? dec : 0u;
+        lv1 |= (level & 2u) ? dec : 0u;
+        lv2 |= (level & 4u) ? dec : 0u;
+        levels = level + 1;
+    }
+    CB_HD uint32_t level_of(uint32_t p) const { return ((lv0 >> p) & 1u) | ((lv1 >> p) & 1u) << 1 | ((lv2 >> p) & 1u) << 2; }
+};
+// Returns true if the request must go to the reference-order body (nothing but DENY effect bytes written then): differing
+// versions, a chain longer than the reference walks, a padding role column before a real role, or what the effect body
+// defers.  side: cbuc::build_meta's records.
+template <typename Cols, typename Rows, typename Conds = GenericConds>
+CB_HD bool eval_request_uc_meta(const TableView t, const BatchView &b, const Cols &cols, const Rows rows, const U4 *side, uint64_t n, uint8_t *effects,
+                                uint32_t *action_meta, cb_request_meta *req_meta, const Conds conds = Conds()) {
+    const U4 h0 = cols.hdr0();
+    const uint64_t h1 = cols.hdr1();
+    const auto regs = conds.load(t, b, cols);
+    const uint32_t pid = h0.x, kc = h0.y, rscope = h0.z, pscope = h0.w;
+    const uint32_t rv = (uint32_t)(h1 & 0xFFFF), pv = (uint32_t)((h1 >> 16) & 0xFFFF), aset = (uint32_t)(h1 >> 32);
+    const uint32_t RC = b.role_cols, RCP = b.rcp, KM = b.max_actions;
+    const uint32_t K = aset < b.n_asets ? cols.aset_k(aset) : 0;
+    uint64_t rp = 0, req_roles = 0;   // role table; the table roles among the request's
+    uint32_t n_roles = 0;
+    bool pad = false, gap = false;    // gap: a padding column before a real role (the reference compacts the roles)
+    for (uint32_t i = 0; i < RC; i++) {
+        const uint32_t rr = cols.role(i);
+        gap |= pad && rr != CB_ROLE_PAD;
+        pad |= rr == CB_ROLE_PAD;
+        n_roles = rr != CB_ROLE_PAD ? i + 1 : n_roles;
+        rp |= rr < t.L->nR ? 1ull << (rr * RCP + i) : 0ull;
+        req_roles |= rr < t.L->nR ? 1ull << rr : 0ull;
+    }
+    if (pv != rv || gap) return true;
+    const bool lenient = (b.flags & CB_BATCH_FLAG_LENIENT) != 0;
+    const uint32_t r0 = chain_start(t, rscope, CB_SCOPE_FLAG_RESOURCE, lenient), p0 = chain_start(t, pscope, CB_SCOPE_FLAG_PRINCIPAL, lenient);
+    const uint32_t bm_base = (rv * t.L->nRP + kc) * t.L->nS;
+    bool exists = false;   // r_exists of the reference
+    if (K != 0 && r0 != CB_NONE32 && rv != CB_NONE16 && kc != CB_KIND_NONE) {
+        const uint32_t w = ld16(side + bm_base + r0).z;   // exists from r0 on | levels from r0 << 8
+        if ((w >> 8) > CB_MAX_CHAIN) return true;
+        exists = (w & 1u) != 0;
+    }
+    const bool walk = exists && n_roles != 0;
+    const uint32_t role_all = (1u << n_roles) - 1;
+    uint32_t allow_pairs = 0, acc = 0;
+    uint64_t edr = 0;
+    UcMetaObserver ob;
+    CondWord val; val.lo = 1; val.hi = 0;
+    if (walk) {
+        bool slow = false;
+        val = conds(t, b, regs, pid, n, slow);
+        if (slow) return true;
+        const uint32_t amask = K * RC >= 32 ? b.stride_pattern : b.stride_pattern & ((1u << (K * RC)) - 1);
+        const uint32_t alive0 = amask * role_all;
+        const Rows arows = rows.aset(t, b, aset);
+        if ((t.L->nR + 1) * RCP <= 32)
+            allow_pairs = uc_walk<Conds::kDenyRows, Conds::kAllowRows, uint32_t, Conds::kForm>(t, arows, (uint32_t)rp | role_all << (t.L->nR * RCP), val, r0, bm_base, role_all, alive0, ob);
+        else allow_pairs = uc_walk<Conds::kDenyRows, Conds::kAllowRows, uint64_t, Conds::kForm>(t, arows, rp | (uint64_t)role_all << (t.L->nR * RCP), val, r0, bm_base, role_all, alive0, ob);
+        // the pairs the reference walks, and the deepest level among them (bit-sliced maximum)
+        uint32_t need = 0;
+        for (uint32_t k = 0; k < K; k++) {
+            const uint32_t a = (allow_pairs >> (k * RC)) & role_all, lowest = a & (0u - a);
+            need |= (lowest ? lowest | (lowest - 1) : role_all) << (k * RC);
+            acc |= (a != 0 ? 1u : 0u) << k;
+        }
+        const uint32_t undecided = alive0 & ~(allow_pairs | ob.deny), last = ob.levels - 1;
+        const uint32_t lv0 = ob.lv0 | ((last & 1u) ? undecided : 0u), lv1 = ob.lv1 | ((last & 2u) ? undecided : 0u), lv2 = ob.lv2 | ((last & 4u) ? undecided : 0u);
+        uint32_t top = 0, cand = need;
+        if (cand & lv2) { top |= 4u; cand &= lv2; }
+        if (cand & lv1) { top |= 2u; cand &= lv1; }
+        if (cand & lv0) top |= 1u;
+        const U4 *chain = t.uc_chain() + bm_base;
+        uint32_t s = r0;
+        for (uint32_t l = 0; l <= top && s != CB_NONE32; l++) {
+            const U4 m = ld16(side + bm_base + s);   // {first derived-role record, end, .., ..}
+            for (uint32_t e = m.x; e < m.y; e++) {
+                const U4 dr = ld16(side + e);        // {name bit, condition | any role << 31, parent roles lo, hi}
+                const bool hit = (dr.y >> 31) != 0 || ((((uint64_t)dr.w << 32) | dr.z) & req_roles) != 0;
+                edr |= (uint64_t)(hit && cond_bit(val, dr.y & 0x7FFFFFFFu)) << dr.x;
+            }
+            s = ld16(chain + s).w;
+        }
+    }
+    store_result(b, cols, n, nullptr, effects, K, acc);
+    uint32_t *am = action_meta + n * (uint64_t)KM;
+    const uint32_t none = walk ? 0xFFFFu | CB_META_SRC_RESOURCE_POLICY << 16 : 0xFFFFu;
+    const U4 *chain = t.uc_chain() + bm_base;
+    for (uint32_t k = 0; k < KM; k++) {
+        uint32_t w = 0xFFFFu;
+        if (k < K) {   // (K * RC <= 32: cbhost::lean_eligible)
+            const uint32_t a = (allow_pairs >> (k * RC)) & role_all, d = (ob.deny >> (k * RC)) & role_all, c = a ? a : d;
+            w = none;
+            if (c) {
+                uint32_t s = r0;
+                for (uint32_t l = 0, lv = ob.level_of(k * RC + ctz32(c)); l < lv; l++) s = ld16(chain + s).w;
+                w = (s & 0xFFFFu) | CB_META_SRC_RESOURCE_POLICY << 16;
+            }
+        }
+        am[k] = w;
+    }
+    cb_request_meta rm;
+    rm.principal_first_scope = (uint16_t)(p0 == CB_NONE32 ? 0xFFFFu : p0);
+    rm.resource_first_scope = (uint16_t)(r0 == CB_NONE32 ? 0xFFFFu : r0);
+    rm.flags = 0;
+    rm.effective_derived_roles = edr;
+    req_meta[n] = rm;
     return false;
 }
 

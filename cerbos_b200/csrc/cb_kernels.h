@@ -302,8 +302,18 @@ __device__ __forceinline__ void check_tiles_body(const TableDesc &td, const cb::
 // versions) go to the launch's deferral list, drained by the general kernel right behind; they are first written as
 // DENY so that a lost deferral could only fail closed.
 // smem layout (kStaged): [image, 128-byte padded][merged rows: n_asets x uc_n_rows (slots or rows) x 16 B]
-template <typename Conds, typename Cols, bool kStaged>
-__device__ __forceinline__ void check_uc_body(const TableDesc &td, const cb::BatchView &bv, uint8_t *bitmap, uint8_t *effects, uint8_t *smem_image, uint64_t *mbar) {
+// Meta: UcMeta -- the metadata form (cb::eval_request_uc_meta: effect bytes, action words and request records; the
+// deferred requests go to the reference-order body, check_meta_kernel), else the effect form.
+struct UcEffects { static constexpr bool kMeta = false; };
+struct UcMeta {
+    static constexpr bool kMeta = true;
+    uint32_t *action_meta;
+    cb_request_meta *req_meta;
+    const cb::U4 *side;   // cbuc::build_meta
+};
+template <typename Conds, typename Cols, bool kStaged, typename Meta = UcEffects>
+__device__ __forceinline__ void check_uc_body(const TableDesc &td, const cb::BatchView &bv, uint8_t *bitmap, uint8_t *effects, uint8_t *smem_image, uint64_t *mbar,
+                                              const Meta meta = Meta()) {
     cb::TableView tv;
     tv.L = &td.lay;
     tv.base = kStaged ? smem_image : td.base;
@@ -356,8 +366,13 @@ __device__ __forceinline__ void check_uc_body(const TableDesc &td, const cb::Bat
             Cols gc;
             gc.b = &bv; gc.n = n;
             bool d;
-            if (kStaged || pk) { cb::UcRowsPacked rows; rows.pk = pk; rows.by_slot = true; d = cb::eval_request_uc(tv, bv, gc, rows, n, bitmap, effects, Conds()); }
-            else { cb::UcRowsGlobal rows; rows.urows = tv.urows(); rows.row_am = bv.row_am; rows.RCP = bv.rcp; rows.nR = td.lay.nR; d = cb::eval_request_uc(tv, bv, gc, rows, n, bitmap, effects, Conds()); }
+            if constexpr (Meta::kMeta) {
+                if (kStaged || pk) { cb::UcRowsPacked rows; rows.pk = pk; rows.by_slot = true; d = cb::eval_request_uc_meta(tv, bv, gc, rows, meta.side, n, effects, meta.action_meta, meta.req_meta, Conds()); }
+                else { cb::UcRowsGlobal rows; rows.urows = tv.urows(); rows.row_am = bv.row_am; rows.RCP = bv.rcp; rows.nR = td.lay.nR; d = cb::eval_request_uc_meta(tv, bv, gc, rows, meta.side, n, effects, meta.action_meta, meta.req_meta, Conds()); }
+            } else {
+                if (kStaged || pk) { cb::UcRowsPacked rows; rows.pk = pk; rows.by_slot = true; d = cb::eval_request_uc(tv, bv, gc, rows, n, bitmap, effects, Conds()); }
+                else { cb::UcRowsGlobal rows; rows.urows = tv.urows(); rows.row_am = bv.row_am; rows.RCP = bv.rcp; rows.nR = td.lay.nR; d = cb::eval_request_uc(tv, bv, gc, rows, n, bitmap, effects, Conds()); }
+            }
             if (d) {
                 cb::store_result(bv, gc, n, bitmap, effects, bv.max_actions, 0u);
                 const uint32_t k = atomicAdd(bv.defer_count, 1u);

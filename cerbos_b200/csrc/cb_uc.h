@@ -226,4 +226,79 @@ inline Image build(const uint8_t *image, const uint32_t *off, const uint64_t *le
     return out;
 }
 
+// Side table of the metadata kernels (cb::eval_request_uc_meta), kept apart from the image so that the effect kernels read
+// the same bytes as without it.  16-byte records:
+//   one per RES_BLOCK_MAP entry (version, kind pattern, scope s), indexed like the chain descriptors:
+//     {first derived-role record, end, bit 0: a resource policy of this kind exists from s to the end of the chain |
+//      scope levels from s to the end of the chain << 8 (saturating at CB_MAX_CHAIN + 1), 0}
+//   then the derived roles of every block the map names (DR_OFF / DR_ENTRIES / DR_PARENTS, in block order):
+//     {name bit, distinct condition number (cond_bit; 0: none) | any parent role << 31, parent-role mask over the table roles (lo, hi)}
+// Only for the tables the unique-condition kernels take whose metadata needs nothing but the resource chain: no principal
+// or role policies, no parent roles (so a parent role matches a request role by equality, cb::role_in_pr), no condition
+// reading runtime.effectiveDerivedRoles, and no principal-policy existence bits.
+struct MetaSide {
+    bool ok = false;
+    std::string why;                // when !ok
+    std::vector<uint32_t> words;    // 4 per record
+};
+
+inline MetaSide build_meta(const uint8_t *image, const uint32_t *off, const uint64_t *len, const uint32_t *meta, const cb::TableLayout &lay, const Image &uc) {
+    MetaSide out;
+    if (!uc.ok) { out.why = "no unique-condition image"; return out; }
+    if (lay.has_principal_policies || lay.has_role_policies || lay.has_parent_roles || lay.uses_runtime) {
+        out.why = "principal / role policies, parent roles or runtime.effectiveDerivedRoles";
+        return out;
+    }
+    const uint32_t nS = lay.nS, n_blocks = meta[CB_META_N_BLOCKS];
+    const uint64_t n_map = (uint64_t)lay.nV * lay.nRP * nS;
+    const uint8_t *pex = image + off[CB_SEC_PRIN_EXISTS];
+    for (uint64_t i = 0; i < (uint64_t)lay.nV * nS; i++)
+        if (pex[i]) { out.why = "principal-policy existence bits"; return out; }
+    const uint32_t *bmap = reinterpret_cast<const uint32_t *>(image + off[CB_SEC_RES_BLOCK_MAP]);
+    const uint8_t *rex = image + off[CB_SEC_RES_EXISTS];
+    const uint32_t *dr_off = reinterpret_cast<const uint32_t *>(image + off[CB_SEC_DR_OFF]);
+    const uint32_t *dr_ent = reinterpret_cast<const uint32_t *>(image + off[CB_SEC_DR_ENTRIES]);
+    const uint32_t *dr_par = reinterpret_cast<const uint32_t *>(image + off[CB_SEC_DR_PARENTS]);
+    const uint64_t n_ent = len[CB_SEC_DR_ENTRIES] / 16, n_par = len[CB_SEC_DR_PARENTS] / 4;
+    const uint32_t *chain = reinterpret_cast<const uint32_t *>(uc.bytes.data() + uc.lay.uc_chain_off);   // {.., .., .., next scope}
+    // scope levels from s to the end of the resource chain
+    std::vector<uint32_t> levels(nS, 0);
+    for (uint32_t s = 0; s < nS; s++) {
+        uint32_t n = 0;
+        for (uint32_t x = s; x != CB_NONE32 && n <= CB_MAX_CHAIN; x = chain[4 * (uint64_t)x + 3]) n++;
+        levels[s] = n;
+    }
+    out.words.assign(4 * n_map, 0);
+    std::vector<uint32_t> first(n_blocks, CB_NONE32), end(n_blocks, 0);   // derived-role records of a block, once emitted
+    for (uint64_t e = 0; e < n_map; e++) {
+        const uint32_t s = (uint32_t)(e % nS), bid = bmap[e];
+        uint32_t exists = 0;
+        for (uint32_t x = s, n = 0; x != CB_NONE32 && n <= CB_MAX_CHAIN; x = chain[4 * (e - s + x) + 3], n++) exists |= rex[e - s + x] & CB_EXISTS_RESOURCE_KIND;
+        out.words[4 * e + 2] = (exists ? 1u : 0u) | levels[s] << 8;
+        if (bid == CB_NONE32) continue;   // (below n_blocks: cbuc::build checked the map)
+        if (first[bid] == CB_NONE32) {
+            first[bid] = (uint32_t)(out.words.size() / 4);
+            if (dr_off[bid] > dr_off[bid + 1] || dr_off[bid + 1] > n_ent) { out.why = "derived-role range out of range"; return out; }
+            for (uint32_t j = dr_off[bid]; j < dr_off[bid + 1]; j++) {
+                const uint32_t *en = dr_ent + 4 * (uint64_t)j;   // {name index, cond + 1, parents start, n parents}
+                if ((uint64_t)en[2] + en[3] > n_par || (en[1] && en[1] - 1 >= uc.ucond_of_gid.size())) { out.why = "derived-role entry out of range"; return out; }
+                uint64_t mask = 0;
+                bool any = false;
+                for (uint32_t q = 0; q < en[3]; q++) {
+                    const uint32_t pr = dr_par[en[2] + q];
+                    if (pr == CB_ROLE_ANY) any = true;
+                    else if (pr < lay.nR) mask |= 1ull << pr;   // (nR <= 64: cbuc::build)
+                }
+                const uint32_t u = en[1] ? uc.ucond_of_gid[en[1] - 1] : 0u;
+                out.words.insert(out.words.end(), {en[0] & 63u, u | (any ? 1u << 31 : 0u), (uint32_t)mask, (uint32_t)(mask >> 32)});
+            }
+            end[bid] = (uint32_t)(out.words.size() / 4);
+        }
+        out.words[4 * e] = first[bid];
+        out.words[4 * e + 1] = end[bid];
+    }
+    out.ok = true;
+    return out;
+}
+
 }  // namespace cbuc

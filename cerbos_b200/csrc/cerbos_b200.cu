@@ -58,10 +58,24 @@ __global__ void __launch_bounds__(kThreads, CB_MIN_BLOCKS) check_kernel_tiles(co
 // decision-metadata kernel (cgpu_check_meta): one thread per request, the reference's own loop order (cb::eval_request_meta)
 // Two resident CTAs (up to 128 registers), stated: left to ptxas, this kernel's register budget moves with the size of the
 // interpreter's call graph, and it fell to 32 registers with heavy spills once the format printers joined it
+// Also the drain of a unique-condition metadata launch (bv.count_dev: the deferral cell, bv.perm: its list), launched in
+// stream order behind it: the last CTA hands the cell back zeroed, as check_body's drain does.
 __global__ void __launch_bounds__(kThreads, 2) check_meta_kernel(const __grid_constant__ TableDesc td, const __grid_constant__ cb::BatchView bv, uint8_t *effects,
                                                              uint32_t *action_meta, cb_request_meta *req_meta, uint32_t *status) {
-    for (uint64_t i = (uint64_t)blockIdx.x * kThreads + threadIdx.x; i < bv.count; i += (uint64_t)gridDim.x * kThreads)
-        cb::eval_request_meta(td.base, &td.lay, &bv, bv.first + i, effects, action_meta, req_meta, status);
+    const uint64_t count = bv.count_dev ? (uint64_t)*bv.count_dev : bv.count;
+    for (uint64_t i = (uint64_t)blockIdx.x * kThreads + threadIdx.x; i < count; i += (uint64_t)gridDim.x * kThreads)
+        cb::eval_request_meta(td.base, &td.lay, &bv, bv.first + (bv.perm ? bv.perm[i] : i), effects, action_meta, req_meta, status);
+    if (bv.count_dev) {
+        __shared__ uint32_t last;
+        __syncthreads();   // every thread of the CTA has read the count
+        if (threadIdx.x == 0) {
+            __threadfence();
+            last = atomicAdd(bv.count_dev + 1, 1u) == gridDim.x - 1;
+            if (blockIdx.x == 0) bv.count_dev[3] += (uint32_t)count;   // the running total of cgpu_deferred_count
+        }
+        __syncthreads();
+        if (last && threadIdx.x == 0) { bv.count_dev[0] = 0; bv.count_dev[1] = 0; }
+    }
 }
 
 // ---- narrow wire format (cgpu_check_narrow): the per-request columns travel over PCIe in their narrowest exact form and are
@@ -181,6 +195,14 @@ __global__ void __launch_bounds__(kThreads, CB_MIN_BLOCKS) check_uc(const __grid
     __shared__ __align__(8) uint64_t mbar;
     (void)status;
     cbk::check_uc_body<cb::GenericConds, cb::CachedCols, kStaged>(td, bv, bitmap, effects, smem_image, &mbar);
+}
+// ... their metadata form (cgpu_check_meta): effects, action words and request records; side: cbuc::build_meta's table
+template <bool kStaged>
+__global__ void __launch_bounds__(kThreads, CB_MIN_BLOCKS) check_uc_meta(const __grid_constant__ TableDesc td, const __grid_constant__ cb::BatchView bv, uint8_t *effects,
+                                                                       uint32_t *action_meta, cb_request_meta *req_meta, const cb::U4 *side) {
+    extern __shared__ __align__(128) uint8_t smem_image[];
+    __shared__ __align__(8) uint64_t mbar;
+    cbk::check_uc_body<cb::GenericConds, cb::CachedCols, kStaged>(td, bv, nullptr, effects, smem_image, &mbar, cbk::UcMeta{action_meta, req_meta, side});
 }
 
 // ------------------------------------------------------------------------------------------------ fused all-gather
@@ -348,8 +370,11 @@ enum class Kernel : uint8_t {
     Uc, UcGlobal,                   // check_uc<true> / <false>
     SpecTiles, SpecDirect,          // cb_spec_tiles / cb_spec_direct (block-shape form)
     SpecUc, SpecUcGlobal,           // cb_spec_uc / cb_spec_uc_global (unique-condition form)
+    // metadata forms of the four unique-condition kernels (cgpu_check_meta): check_uc_meta<true> / <false>,
+    // cb_spec_uc_meta / cb_spec_uc_meta_global
+    UcMeta, UcMetaGlobal, SpecUcMeta, SpecUcMetaGlobal,
 };
-constexpr int kKernels = (int)Kernel::SpecUcGlobal + 1;
+constexpr int kKernels = (int)Kernel::SpecUcMetaGlobal + 1;
 
 // What one check launch runs: plan_launch decides it, launch_check executes it.
 struct LaunchPlan {
@@ -472,6 +497,7 @@ struct cgpu_table {
     std::atomic<int> spec_state{0};   // 0 not tried, 1 ready, -1 unavailable
     cudaLibrary_t spec_lib = nullptr;
     cudaKernel_t spec_tiles = nullptr, spec_direct = nullptr, spec_uc = nullptr, spec_uc_global = nullptr, spec_strpred = nullptr;
+    cudaKernel_t spec_uc_meta = nullptr, spec_uc_meta_global = nullptr;
     uint32_t spec_n_strpred = 0;   // string predicates the specialised unique-condition kernel reads from the per-string pre-pass
     std::string spec_note;
     // unique-condition image (cb_uc.h): compact copy of the table for tables whose blocks differ in shape
@@ -480,6 +506,8 @@ struct cgpu_table {
     cbuc::Image uc;
     uint8_t *d_uc_image = nullptr;
     TableDesc uc_desc{};
+    cbuc::MetaSide uc_meta;            // side table of the metadata forms of the unique-condition kernels (cb_uc.h: build_meta)
+    cb::U4 *d_uc_meta = nullptr;       // (own allocation: the image the effect kernels read stays as it is)
     std::thread spec_thread;          // compiles the specialised kernels in the background from cgpu_table_load on
     std::mutex join_mu;
 };
@@ -554,6 +582,19 @@ const char kSpecUcGlobal[] =
     "\nextern \"C\" __global__ void __launch_bounds__(256, CB_SPEC_UC_MIN_BLOCKS) cb_spec_uc_global(const __grid_constant__ cbk::TableDesc td, const __grid_constant__ cb::BatchView bv,\n"
     "        uint8_t *bitmap, uint8_t *effects, uint32_t *status, const uint32_t) {\n"
     "    cbk::check_uc_body<cb::SpecConds, cb::GlobalCols, false>(td, bv, bitmap, effects, nullptr, nullptr);\n"
+    "}\n";
+// metadata forms of the two (cgpu_check_meta; side: cbuc::build_meta's table)
+const char kSpecUcMetaStaged[] =
+    "\nextern \"C\" __global__ void __launch_bounds__(256, CB_SPEC_UC_MIN_BLOCKS) cb_spec_uc_meta(const __grid_constant__ cbk::TableDesc td, const __grid_constant__ cb::BatchView bv,\n"
+    "        uint8_t *effects, uint32_t *action_meta, cb_request_meta *req_meta, const cb::U4 *side) {\n"
+    "    extern __shared__ __align__(128) uint8_t smem_image[];\n"
+    "    __shared__ __align__(8) uint64_t mbar;\n"
+    "    cbk::check_uc_body<cb::SpecConds, cb::GlobalCols, true>(td, bv, nullptr, effects, smem_image, &mbar, cbk::UcMeta{action_meta, req_meta, side});\n"
+    "}\n";
+const char kSpecUcMetaGlobal[] =
+    "\nextern \"C\" __global__ void __launch_bounds__(256, CB_SPEC_UC_MIN_BLOCKS) cb_spec_uc_meta_global(const __grid_constant__ cbk::TableDesc td, const __grid_constant__ cb::BatchView bv,\n"
+    "        uint8_t *effects, uint32_t *action_meta, cb_request_meta *req_meta, const cb::U4 *side) {\n"
+    "    cbk::check_uc_body<cb::SpecConds, cb::GlobalCols, false>(td, bv, nullptr, effects, nullptr, nullptr, cbk::UcMeta{action_meta, req_meta, side});\n"
     "}\n";
 // pre-pass over the string dictionary (table strings, then the batch's): one predicate word per string
 const char kSpecUcStrpred[] =
@@ -656,8 +697,9 @@ SpecForm spec_compile(const uint8_t *image, const cb::TableLayout &lay, const ui
     if (form == SPEC_UC) {
         // an image that can never be staged (larger than the shared-memory budget of the staged kernel) gets the global
         // variant only, a small one both: which of the two a launch takes also depends on the batch's action sets
-        if (uc_stageable(uc)) src += kSpecUcStaged;
+        if (uc_stageable(uc)) { src += kSpecUcStaged; src += kSpecUcMetaStaged; }
         src += kSpecUcGlobal;
+        src += kSpecUcMetaGlobal;
         src += kSpecUcStrpred;
     } else src += kSpecKernels;
     const char *mb = getenv("CERBOS_B200_SPEC_BLOCKS");   // experiments: resident CTAs / SM the specialised kernels are budgeted for
@@ -722,8 +764,10 @@ bool ensure_spec(cgpu_ctx *ctx, cgpu_table *t) {
     const SpecForm form = spec_compile(t->host_image.data(), t->desc.lay, t->meta, t->uc, &cubin, &why, &t->spec_n_strpred);
     if (form == SPEC_NONE) return give_up(why);
     if (cudaLibraryLoadData(&t->spec_lib, cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0) != cudaSuccess) { cudaGetLastError(); return give_up("cudaLibraryLoadData failed"); }
-    bool got = form == SPEC_UC ? (!uc_stageable(t->uc) || cudaLibraryGetKernel(&t->spec_uc, t->spec_lib, "cb_spec_uc") == cudaSuccess) &&
+    bool got = form == SPEC_UC ? (!uc_stageable(t->uc) || (cudaLibraryGetKernel(&t->spec_uc, t->spec_lib, "cb_spec_uc") == cudaSuccess &&
+                                                            cudaLibraryGetKernel(&t->spec_uc_meta, t->spec_lib, "cb_spec_uc_meta") == cudaSuccess)) &&
                                      cudaLibraryGetKernel(&t->spec_uc_global, t->spec_lib, "cb_spec_uc_global") == cudaSuccess &&
+                                     cudaLibraryGetKernel(&t->spec_uc_meta_global, t->spec_lib, "cb_spec_uc_meta_global") == cudaSuccess &&
                                      cudaLibraryGetKernel(&t->spec_strpred, t->spec_lib, "cb_spec_strpred") == cudaSuccess
                                : cudaLibraryGetKernel(&t->spec_tiles, t->spec_lib, "cb_spec_tiles") == cudaSuccess &&
                                      cudaLibraryGetKernel(&t->spec_direct, t->spec_lib, "cb_spec_direct") == cudaSuccess;
@@ -732,6 +776,7 @@ bool ensure_spec(cgpu_ctx *ctx, cgpu_table *t) {
         cudaLibraryUnload(t->spec_lib);
         t->spec_lib = nullptr;
         t->spec_tiles = t->spec_direct = t->spec_uc = t->spec_uc_global = t->spec_strpred = nullptr;
+        t->spec_uc_meta = t->spec_uc_meta_global = nullptr;
         return give_up("cudaLibraryGetKernel failed");
     }
     t->spec_note = "ok";
@@ -863,9 +908,23 @@ const void *kernel_fn(const cgpu_table &t, Kernel k) {
     case Kernel::SpecDirect: return (const void *)t.spec_direct;
     case Kernel::SpecUc: return (const void *)t.spec_uc;
     case Kernel::SpecUcGlobal: return (const void *)t.spec_uc_global;
+    case Kernel::UcMeta: return (const void *)check_uc_meta<true>;
+    case Kernel::UcMetaGlobal: return (const void *)check_uc_meta<false>;
+    case Kernel::SpecUcMeta: return (const void *)t.spec_uc_meta;
+    case Kernel::SpecUcMetaGlobal: return (const void *)t.spec_uc_meta_global;
     }
     return nullptr;
 }
+// the metadata form of a unique-condition kernel
+Kernel meta_kernel(Kernel k) {
+    return k == Kernel::Uc ? Kernel::UcMeta : k == Kernel::UcGlobal ? Kernel::UcMetaGlobal : k == Kernel::SpecUc ? Kernel::SpecUcMeta : Kernel::SpecUcMetaGlobal;
+}
+
+// The device outputs of a metadata launch (cgpu_check_meta) beyond the effect bytes.
+struct MetaDev {
+    uint32_t *action_meta;
+    cb_request_meta *req_meta;
+};
 
 // Resident CTAs per SM of kernel k with `smem` bytes of dynamic shared memory, queried once per (table, kernel, footprint);
 // also lifts the kernel's dynamic shared-memory limit to kMaxStageBytes.  A CGPU_ERR_* code (< 0) when the query fails.
@@ -877,7 +936,7 @@ int resident_ctas(const cgpu_table &t, Kernel k, uint32_t smem) {
     int occ = 0;
     if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxStageBytes) != cudaSuccess ||
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, kThreads, smem) != cudaSuccess) {
-        if (k < Kernel::SpecTiles) return fail(CGPU_ERR_CUDA, "kernel attribute / occupancy query failed: %s", cudaGetErrorString(cudaGetLastError()));
+        if (k < Kernel::SpecTiles || k == Kernel::UcMeta || k == Kernel::UcMetaGlobal) return fail(CGPU_ERR_CUDA, "kernel attribute / occupancy query failed: %s", cudaGetErrorString(cudaGetLastError()));
         cudaGetLastError();
         occ = CB_MIN_BLOCKS;   // run-time loaded kernel on a runtime that cannot query it: the launch-bounds minimum
     }
@@ -898,9 +957,12 @@ cudaError_t launch_serialised(const void *fn, uint32_t grid, uint32_t block, uin
     return cudaLaunchKernelExC(&cfg, fn, args);
 }
 
-// Issues the launches of `plan` (plan_launch for this table and batch) on `stream`.
-int launch_check(cgpu_ctx *ctx, const cgpu_table *t, const LaunchPlan &plan, const cb::BatchView &bv, uint8_t *d_bitmap, uint8_t *d_effects,
-                 uint32_t *d_status, cudaStream_t stream) {
+// Issues the launches of `plan` (plan_launch for this table and batch) on `stream`.  md: the metadata form of the plan's
+// unique-condition kernel (cbuc::build_meta's table must exist), its deferrals drained by check_meta_kernel.
+int launch_check(cgpu_ctx *ctx, const cgpu_table *t, const LaunchPlan &plan_in, const cb::BatchView &bv, uint8_t *d_bitmap, uint8_t *d_effects,
+                 uint32_t *d_status, cudaStream_t stream, const MetaDev *md = nullptr) {
+    LaunchPlan plan = plan_in;
+    if (md) plan.kernel = meta_kernel(plan.kernel);
     const cb::TableLayout &lay = t->desc.lay;
     const uint64_t tiles = (bv.count + kThreads - 1) / kThreads;
     const int occ = resident_ctas(*t, plan.kernel, plan.smem);
@@ -950,6 +1012,10 @@ int launch_check(cgpu_ctx *ctx, const cgpu_table *t, const LaunchPlan &plan, con
     }
     const void *fn = kernel_fn(*t, plan.kernel);
     void *args[] = {&td, &bvv, &d_bitmap, &d_effects, &d_status, &last_arg};
+    uint32_t *d_am = md ? md->action_meta : nullptr;
+    cb_request_meta *d_rm = md ? md->req_meta : nullptr;
+    const cb::U4 *d_side = t->d_uc_meta;
+    void *margs[] = {&td, &bvv, &d_effects, &d_am, &d_rm, &d_side};
     if (ctx->profiling) {
         if (ctx->prof_pending && cudaEventSynchronize(ctx->ev1) == cudaSuccess) {
             float ms = 0;
@@ -964,11 +1030,20 @@ int launch_check(cgpu_ctx *ctx, const cgpu_table *t, const LaunchPlan &plan, con
         // It reads nothing the previous launch writes.
         CUDA_TRY(launch_serialised(fn, grid, kThreads, plan.smem, stream, args));
     } else {
-        CUDA_TRY(cudaLaunchKernel(fn, dim3(grid), dim3(kThreads), args, plan.smem, stream));
+        CUDA_TRY(cudaLaunchKernel(fn, dim3(grid), dim3(kThreads), md ? margs : args, plan.smem, stream));
     }
     CUDA_TRY(cudaGetLastError());
     if (ctx->profiling) { CUDA_TRY(cudaEventRecord(ctx->ev1, stream)); ctx->prof_pending = true; }
-    if (plan.lean) {
+    if (md) {
+        // drain the deferral list with the reference-order metadata body, in stream order (it has no programmatic wait)
+        cb::BatchView dv = bv;
+        dv.perm = defer;
+        dv.count_dev = bvv.defer_count;
+        const uint64_t gmax = (uint64_t)ctx->sm_count * 4;
+        check_meta_kernel<<<(unsigned)(tiles < gmax ? tiles : gmax), kThreads, 0, stream>>>(t->desc, dv, d_effects, d_am, d_rm, d_status);
+        CUDA_TRY(cudaGetLastError());
+        ctx->launches.fetch_add(1, std::memory_order_relaxed);
+    } else if (plan.lean) {
         // drain the deferral list with the general body (usually empty: the kernel then exits at once); it also does the
         // fused-gather signalling (BatchView::sig_*)
         cb::BatchView dv = bv;
@@ -1108,10 +1183,16 @@ int cgpu_table_load(cgpu_ctx *ctx, const void *blob, size_t len, cgpu_table **ou
     if (e == cudaSuccess && t->uc.ok) {
         e = cudaMalloc(reinterpret_cast<void **>(&t->d_uc_image), t->uc.bytes.size());
         if (e == cudaSuccess) e = cudaMemcpy(t->d_uc_image, t->uc.bytes.data(), t->uc.bytes.size(), cudaMemcpyHostToDevice);
+        t->uc_meta = cbuc::build_meta(static_cast<const uint8_t *>(blob), t->desc.lay.off, t->sec_len, t->meta, t->desc.lay, t->uc);
+        if (e == cudaSuccess && t->uc_meta.ok) {
+            e = cudaMalloc(reinterpret_cast<void **>(&t->d_uc_meta), t->uc_meta.words.size() * 4);
+            if (e == cudaSuccess) e = cudaMemcpy(t->d_uc_meta, t->uc_meta.words.data(), t->uc_meta.words.size() * 4, cudaMemcpyHostToDevice);
+        }
     }
     if (e != cudaSuccess) {
         if (t->d_image) cudaFree(t->d_image);
         if (t->d_uc_image) cudaFree(t->d_uc_image);
+        if (t->d_uc_meta) cudaFree(t->d_uc_meta);
         delete t;
         return fail(CGPU_ERR_CUDA, "table upload failed: %s", cudaGetErrorString(e));
     }
@@ -1149,6 +1230,7 @@ void cgpu_table_release(cgpu_table *t) {
         cudaDeviceSynchronize();   // no kernel may still read the image
         cudaFree(t->d_image);
         if (t->d_uc_image) cudaFree(t->d_uc_image);
+        if (t->d_uc_meta) cudaFree(t->d_uc_meta);
         if (t->spec_lib) cudaLibraryUnload(t->spec_lib);
         delete t;
     }
@@ -1810,11 +1892,22 @@ static int check_range(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *bat
         cv.first = c0; cv.count = cnt;
         // the kernel writes effect bytes directly (1 ALLOW / 2 DENY / 0 padding): no host post-pass
         if (meta) {
-            const uint64_t tiles = (cnt + kThreads - 1) / kThreads;
-            const uint32_t grid = (uint32_t)(tiles < (uint64_t)ctx->sm_count * 4 ? tiles : (uint64_t)ctx->sm_count * 4);
-            check_meta_kernel<<<grid, kThreads, 0, slot->stream>>>(t->desc, cv, d_effects, d_am, d_rm, slot->d_status);
-            CUDA_TRY(cudaGetLastError());
-            ctx->launches.fetch_add(1, std::memory_order_relaxed);
+            // the unique-condition kernel the effect launch would run, in its metadata form, where the table has the side
+            // table that form reads; else the reference-order body for every request
+            const LaunchPlan plan = plan_launch(*ctx, *t, cv);
+            if (plan.uc && t->d_uc_meta) {
+                const MetaDev md{d_am, d_rm};
+                rc = launch_check(ctx, t, plan, cv, nullptr, d_effects, slot->d_status, slot->stream, &md);
+                if (rc != CGPU_OK) return rc;
+            } else {
+                const uint64_t tiles = (cnt + kThreads - 1) / kThreads;
+                const uint32_t grid = (uint32_t)(tiles < (uint64_t)ctx->sm_count * 4 ? tiles : (uint64_t)ctx->sm_count * 4);
+                check_meta_kernel<<<grid, kThreads, 0, slot->stream>>>(t->desc, cv, d_effects, d_am, d_rm, slot->d_status);
+                CUDA_TRY(cudaGetLastError());
+                ctx->launches.fetch_add(1, std::memory_order_relaxed);
+                ctx->last_plan = LaunchPlan();   // (general body, no unique-condition kernel)
+                ctx->last_grid = grid;
+            }
         } else {
             rc = launch_check(ctx, t, plan_launch(*ctx, *t, cv), cv, nullptr, d_effects, slot->d_status, slot->stream);
             if (rc != CGPU_OK) return rc;

@@ -2,7 +2,7 @@
 """What the unique-condition kernels of one workload compile to, without a device.
 
 Generates the workload table's run-time specialised translation unit and compiles it with NVRTC exactly as a table
-load does (capi.compile_check), then prints for cb_spec_uc / cb_spec_uc_global: registers and stack, the SASS
+load does (capi.compile_check), then prints for cb_spec_uc / cb_spec_uc_global and their metadata forms: registers and stack, the SASS
 instruction count, the part of it inlined from cb::eval_request_uc (the per-request path), the generic byte loads
 (LD.E.U8), the local-memory loads and stores (LDL / STL) and the instruction count per source function (the innermost function of each instruction's line info,
 nvdisasm -gi).  Needs the built library and the CUDA toolkit's cuobjdump / nvdisasm.
@@ -21,7 +21,7 @@ import tempfile
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-KERNELS = ("cb_spec_uc", "cb_spec_uc_global")
+KERNELS = ("cb_spec_uc", "cb_spec_uc_global", "cb_spec_uc_meta", "cb_spec_uc_meta_global")
 _DEF = re.compile(r"^\s*(?:template\s*<[^>]*>\s*)?(?:static\s+)?(?:CB_HD_NOINLINE|CB_HD|__device__[\w\s]*|inline)\b[^;=]*?(\boperator\(\)|\b\w+)\s*\(")
 _LINE = re.compile(r'//## File "[^"]*", line (\d+)')
 _INSN = re.compile(r"^\s+/\*[0-9a-f]+\*/\s+(.*?)\s*;")

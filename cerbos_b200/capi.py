@@ -16,7 +16,7 @@ OK, ERR_INVALID, ERR_CUDA, ERR_UNSUPPORTED, ERR_NO_DEVICE = 0, -1, -2, -3, -4
 
 EXPORTS = [
     "cgpu_init", "cgpu_shutdown", "cgpu_table_load", "cgpu_table_retain", "cgpu_table_release", "cgpu_check", "cgpu_check_meta", "cgpu_check_narrow",
-    "cgpu_check_narrow_meta",
+    "cgpu_check_narrow_meta", "cgpu_check_outputs",
     "cgpu_check_device", "cgpu_sync", "cgpu_launch_count", "cgpu_deferred_count", "cgpu_table_info", "cgpu_last_kernel_config",
     "cgpu_last_cluster_config", "cgpu_profile", "cgpu_table_wait_ready", "cgpu_table_compile_check", "cgpu_peer_alloc", "cgpu_peer_open", "cgpu_peer_close",
     "cgpu_peer_free", "cgpu_peer_read", "cgpu_check_device_gather", "cgpu_gather_wait", "cgpu_last_error",
@@ -78,6 +78,9 @@ def lib():
         L.cgpu_check_narrow.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(_Batch), ctypes.POINTER(_Narrow), ctypes.c_void_p]
         L.cgpu_check_meta.restype = ctypes.c_int
         L.cgpu_check_meta.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(_Batch), ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
+        L.cgpu_check_outputs.restype = ctypes.c_int
+        L.cgpu_check_outputs.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(_Batch), ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                         ctypes.c_void_p, ctypes.c_uint32, ctypes.POINTER(ctypes.c_uint32)]
         L.cgpu_check_narrow_meta.restype = ctypes.c_int
         L.cgpu_check_narrow_meta.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(_Batch), ctypes.POINTER(_Narrow), ctypes.c_void_p,
                                              ctypes.c_void_p, ctypes.c_void_p]
@@ -401,6 +404,29 @@ class Table:
         _check(lib().cgpu_check_meta(self.ctx._h, self._h, ctypes.byref(b), eff.ctypes.data_as(ctypes.c_void_p),
                                      am.ctypes.data_as(ctypes.c_void_p), rm.ctypes.data_as(ctypes.c_void_p)))
         return eff, am, rm
+
+    def check_outputs(self, columns, n: int, max_actions: int, stride: int, now_ns: int = 0, flags: int = 0):
+        """cgpu_check_outputs: check_meta's three outputs + the output records uint8[n, stride] (decode with
+        cerbos_b200.outputs) + the size a record that did not fit needed (0 when all fit).  A failure raises CgpuError;
+        after a record overflow its `bytes_needed` is that size."""
+        from .meta import REQUEST_META_DTYPE
+        cols = [c if (isinstance(c, np.ndarray) and c.flags["C_CONTIGUOUS"]) else np.ascontiguousarray(c) for c in columns]
+        ptrs = (ctypes.c_void_p * len(cols))(*[c.ctypes.data for c in cols])
+        sizes = (ctypes.c_size_t * len(cols))(*[c.nbytes for c in cols])
+        b = _Batch(n, max_actions, now_ns, flags, ptrs, sizes, len(cols))
+        km = max(max_actions, 1)
+        eff = np.empty((n, km), dtype=np.uint8)
+        am = np.empty((n, km), dtype=np.uint32)
+        rm = np.empty(n, dtype=REQUEST_META_DTYPE)
+        rec = np.empty((n, stride), dtype=np.uint8)
+        need = ctypes.c_uint32(0)
+        rc = lib().cgpu_check_outputs(self.ctx._h, self._h, ctypes.byref(b), eff.ctypes.data_as(ctypes.c_void_p), am.ctypes.data_as(ctypes.c_void_p),
+                                      rm.ctypes.data_as(ctypes.c_void_p), rec.ctypes.data_as(ctypes.c_void_p), ctypes.c_uint32(stride), ctypes.byref(need))
+        if rc != OK:
+            err = CgpuError(rc, lib().cgpu_last_error().decode("utf-8", "replace"))
+            err.bytes_needed = need.value
+            raise err
+        return eff, am, rm, rec, need.value
 
     def check_narrow_meta(self, nb, now_ns: int = 0, flags: int = 0):
         """cgpu_check_narrow_meta: check_meta's three outputs from a batch in the narrow wire form -- a

@@ -40,7 +40,7 @@ struct alignas(16) U4 { uint32_t x, y, z, w; };
 // Section offsets + dimensions of the table image.  In the kernels this lives in the (grid-constant) kernel
 // parameters, so reading a field is a constant-bank operand and costs no register.
 struct TableLayout {
-    uint32_t off[32];   // by section id (CB_SEC_*)
+    uint32_t off[CB_IMAGE_SECTIONS];   // by section id (CB_SEC_*); 0: the section is absent
     uint32_t nV, nRP, nS, nP, nR, nAP, nT, n_slots, n_rows;
     uint32_t has_role_policies, has_parent_roles, has_principal_policies;
     uint32_t image_bytes;
@@ -87,6 +87,8 @@ struct TableView {
     CB_HD const uint32_t *dr_entries() const { return sec<uint32_t>(CB_SEC_DR_ENTRIES); }   // 4 words each
     CB_HD const uint32_t *dr_parents() const { return sec<uint32_t>(CB_SEC_DR_PARENTS); }
     CB_HD const uint32_t *dr_name_str() const { return sec<uint32_t>(CB_SEC_DR_NAME_STR); }
+    CB_HD const uint32_t *row_out() const { return sec<uint32_t>(CB_SEC_ROW_OUT); }            // tables with rule outputs only
+    CB_HD const cb_out_entry *out_entries() const { return sec<cb_out_entry>(CB_SEC_OUT_ENTRIES); }
     CB_HD const cb_cond *uconds() const { return reinterpret_cast<const cb_cond *>(base + L->uc_conds_off); }     // [n_uconds + 1]; entry 0: {rows of the longest scope, 0, 0, 0} (cb_uc.h)
     CB_HD const U4 *urows() const { return reinterpret_cast<const U4 *>(base + L->uc_rows_off); }                 // [n_rows] 16-byte rows, DENY first per block
     CB_HD const uint32_t *uc_slots() const { return reinterpret_cast<const uint32_t *>(base + L->uc_slots_off); }  // [uc_n_rows] segment form: image row per slot
@@ -3149,9 +3151,13 @@ CB_HD bool cond_true(const Val &v) { return v.tag == CB_T_BOOL && v.u == 1; }
 #endif  // !CB_LEAN_ONLY || CB_SPEC_PROGRAMS
 
 #ifndef CB_LEAN_ONLY   // the stack interpreter
-// Runs one condition program; returns true iff it yields BOOL true (ruletable.go:1425-1441).
-CB_HD_NOINLINE bool run_program(Ctx &c, const cb_instr *code) {
-    Val st[CB_MAX_STACK + 1];
+// Runs one condition program; returns true iff it yields BOOL true (ruletable.go:1425-1441).  run_program<true>(c, code, &v)
+// also hands back the program's value (a rule output, with the deeper value-program stack); the condition form takes no
+// out-pointer, so its code is the interpreter's alone.
+template <bool VALUE = false, typename... Out>
+CB_HD_NOINLINE bool run_program(Ctx &c, const cb_instr *code, Out... out) {
+    static_assert(sizeof...(Out) == (VALUE ? 1 : 0), "run_program<true> takes one Val *");
+    Val st[(VALUE ? CB_OUT_MAX_STACK : CB_MAX_STACK) + 1];
     Loop loops[CB_MAX_LOOP_DEPTH];
     int sp = 0, ld = 0;
     uint32_t pc = 0;
@@ -3162,7 +3168,9 @@ CB_HD_NOINLINE bool run_program(Ctx &c, const cb_instr *code) {
         uint32_t op = (uint32_t)(raw & 0xFF), ia = (uint32_t)((raw >> 8) & 0xFF), ib = (uint32_t)((raw >> 16) & 0xFFFF);
         uint32_t ic = (uint32_t)(raw >> 32);
         switch (op) {
-        case CB_OP_RET: return cond_true(st[sp - 1]);
+        case CB_OP_RET:
+            if constexpr (VALUE) ((*out = st[sp - 1]), ...);
+            return cond_true(st[sp - 1]);
         case CB_OP_CONST: st[sp++] = load_const(c, ic); break;
         case CB_OP_SLOT: { int s; st[sp++] = load_slot(c, ic, &s); break; }
         case CB_OP_HAS_SLOT: { int s; load_slot(c, ic, &s); st[sp++] = op_has_slot(s); break; }
@@ -3469,6 +3477,110 @@ CB_HD_NOINLINE uint32_t cond_sat_code(const uint8_t *base, const TableLayout *L,
     bool s = run_program(c, t.code() + code_off);
     return (s ? 1u : 0u) | (c.unsupported ? 2u : 0u);
 }
+
+// ---------------------------------------------------------------------------------------------- rule outputs
+// Writes a request's output record (layout.py: OUT_TAGS): bytes at and past `cap` are counted, never written, so that a
+// record that does not fit still reports the size it needs.
+struct OutWriter {
+    uint8_t *p;
+    uint32_t cap, pos;
+    CB_HD void put8(uint32_t x) { if (pos < cap) p[pos] = (uint8_t)x; pos++; }
+    CB_HD void put32(uint32_t x) { for (int i = 0; i < 4; i++) put8(x >> (8 * i)); }
+    CB_HD void put64(uint64_t x) { for (int i = 0; i < 8; i++) put8((uint32_t)(x >> (8 * i))); }
+};
+
+// Serialises v (strings and containers of the table, the batch or the arena) depth first with an explicit stack of
+// (container, next item) frames; nesting deeper than CB_OUT_MAX_DEPTH sets `unsupported`.
+CB_HD void out_value(Ctx &c, OutWriter &w, Val v) {
+    struct Frame { const uint64_t *p; uint32_t n, i, items; } st[CB_OUT_MAX_DEPTH];
+    int d = 0;
+    for (;;) {
+        switch (v.tag) {
+        case CB_T_ERR: w.put8(CB_OUT_NO_VALUE); break;
+        case CB_T_NULL: w.put8(CB_OUT_NULL); break;
+        case CB_T_BOOL: w.put8(CB_OUT_BOOL); w.put8((uint32_t)(v.u & 1)); break;
+        case CB_T_INT: w.put8(CB_OUT_INT); w.put64(v.u); break;
+        case CB_T_UINT: w.put8(CB_OUT_UINT); w.put64(v.u); break;
+        case CB_T_DOUBLE: w.put8(CB_OUT_DOUBLE); w.put64(v.u); break;
+        case CB_T_TS: w.put8(CB_OUT_TIMESTAMP); w.put64(v.u); break;
+        case CB_T_DUR: w.put8(CB_OUT_DURATION); w.put64(v.u); break;
+        case CB_T_STRING: case CB_T_BYTES: {
+            const uint8_t *sp; uint32_t len;
+            str_get(c, v.u, sp, len);
+            w.put8(v.tag == CB_T_STRING ? CB_OUT_STRING : CB_OUT_BYTES);
+            w.put32(len);
+            for (uint32_t i = 0; i < len; i++) w.put8(ldg(sp + i));
+            break;
+        }
+        case CB_T_LIST: case CB_T_MAP: {
+            if (d == CB_OUT_MAX_DEPTH) { c.unsupported = 1; return; }
+            const uint64_t *hp = heap_ptr(c, v.u);
+            const uint32_t n = (uint32_t)ldg(hp);
+            w.put8(v.tag == CB_T_LIST ? CB_OUT_LIST : CB_OUT_MAP);
+            w.put32(n);
+            st[d].p = hp; st[d].n = n; st[d].i = 0; st[d].items = v.tag == CB_T_LIST ? n : 2 * n;
+            d++;
+            break;
+        }
+        default: w.put8(CB_OUT_NOT_CONVERTIBLE); break;   // type values, SPIFFE ids: no google.protobuf.Value form
+        }
+        for (;;) {   // the next item: list elements in order; map entries as key, value (keys at [1, n], values at [n + 1, 2n])
+            if (d == 0) return;
+            Frame &f = st[d - 1];
+            if (f.i < f.items) {
+                const uint32_t j = f.i++;
+                const uint64_t at = f.items == f.n ? 1 + j : (j & 1) ? 1 + f.n + j / 2 : 1 + j / 2;
+                v = decode_elem(ldg(f.p + at));
+                break;
+            }
+            d--;
+        }
+    }
+}
+
+// Evaluates the output program at `code_off` and appends its entry {action, src, value} at `pos` of the record `rec` (`cap`
+// bytes): the value is serialised while the program's arena still holds it.  Returns the new position | unsupported << 32.
+// Scalar arguments only, like cond_sat.
+CB_HD_NOINLINE uint64_t emit_output(const uint8_t *base, const TableLayout *L, const BatchView *b, uint64_t req, uint32_t pid, uint64_t edr,
+                                    uint32_t code_off, uint32_t src, uint32_t action, uint8_t *rec, uint32_t cap, uint32_t pos) {
+    TableView t; t.base = base; t.L = L;
+    Ctx c;
+    c.t = &t; c.b = b; c.req = req; c.pid = pid; c.unsupported = 0; c.scr_used = 0; c.edr = edr;
+    Val v = mk_err();
+    run_program<true>(c, t.code() + code_off, &v);
+    OutWriter w; w.p = rec; w.cap = cap; w.pos = pos;
+    w.put8(action & 0xFF); w.put8((action >> 8) & 0xFF); w.put8(0); w.put8(0);
+    w.put32(src);
+    out_value(c, w, v);
+    return w.pos | (c.unsupported ? 1ull << 32 : 0ull);
+}
+
+// Output sinks of the reference-order walk (eval_request_meta / eval_request_outputs): told of every visited row with its
+// condition's outcome.  NoOutputs compiles away; OutputSink emits the row's activated / not-met entry, if it has one.
+struct NoOutputs {
+    static constexpr bool kOn = false;
+    CB_HD void row(const uint8_t *, const TableLayout *, const BatchView *, uint64_t, uint32_t, uint64_t, uint32_t, uint32_t, bool) {}
+};
+enum { CB_OUT_STATUS_OVERFLOW = 2, CB_OUT_STATUS_UNLOWERED = 4 };   // status bits of cgpu_check_outputs (bit 0: unsupported value)
+struct OutputSink {
+    static constexpr bool kOn = true;
+    uint8_t *rec;
+    uint32_t cap, pos, count, status;
+    CB_HD void row(const uint8_t *base, const TableLayout *L, const BatchView *b, uint64_t n, uint32_t pid, uint64_t edr, uint32_t rix, uint32_t k, bool sat) {
+        if (!L->off[CB_SEC_ROW_OUT]) return;
+        TableView t; t.base = base; t.L = L;
+        const uint32_t e = ldg(t.row_out() + rix);
+        if (e == CB_NONE32) return;
+        const U4 en = ld16(t.out_entries() + e);   // {src, activated, not met, flags}
+        if (en.w & (sat ? CB_OUT_UNLOWERED_ACTIVATED : CB_OUT_UNLOWERED_NOT_MET)) { status |= CB_OUT_STATUS_UNLOWERED; return; }
+        const uint32_t off = sat ? en.y : en.z;
+        if (off == CB_NONE32) return;
+        const uint64_t r = emit_output(base, L, b, n, pid, edr, off, en.x, k, rec, cap, pos);
+        pos = (uint32_t)r;
+        status |= (uint32_t)(r >> 32);
+        count++;
+    }
+};
 
 #endif  // !CB_LEAN_ONLY
 
@@ -4347,8 +4459,20 @@ CB_HD bool meta_row_action(const BatchView &b, uint32_t aset, uint32_t n_rows, u
     return ((ldg(b.row_am + ((uint64_t)ps * b.n_asets + aset) * n_rows + ri) >> (kk * b.role_cols)) & 1) != 0;
 }
 
-CB_HD_NOINLINE void eval_request_meta(const uint8_t *base, const TableLayout *L, const BatchView *bp, uint64_t n, uint8_t *effects, uint32_t *action_meta,
-                                      cb_request_meta *req_meta, uint32_t *status) {
+// The smallest action index j <= k whose action row `rix` matches (it matches k): the reference gathers a scope's candidate
+// rows action by action (index.go:564-801), so a row that matches an earlier action of the request is visited earlier.
+CB_HD uint32_t first_action(const BatchView &b, uint32_t aset, uint32_t n_rows, uint32_t rix, uint32_t k) {
+    uint32_t j = 0;
+    while (j < k && !meta_row_action(b, aset, n_rows, j / b.kc, j % b.kc, rix)) j++;
+    return j;
+}
+
+// The reference-order walk, told to an output sink at every visited row (NoOutputs: the metadata body alone).  With outputs
+// on, each scope's rows are visited in the reference's candidate order -- grouped by the first request action they match --
+// since a satisfied DENY ends the walk and outputs show which rows were reached.
+template <class Sink>
+CB_HD void walk_request(const uint8_t *base, const TableLayout *L, const BatchView *bp, uint64_t n, uint8_t *effects, uint32_t *action_meta,
+                        cb_request_meta *req_meta, uint32_t *status, Sink &sink) {
     TableView t; t.base = base; t.L = L;
     const BatchView &b = *bp;
     const U4 h0 = ldcol128(b.hdr0 + n);
@@ -4431,12 +4555,16 @@ CB_HD_NOINLINE void eval_request_meta(const uint8_t *base, const TableLayout *L,
                         const uint32_t bid = (pidx != CB_NONE32 && rows_ok) ? ldg(t.prin_block_map() + ((uint64_t)rv * L->nP + pidx) * L->nS + s) : CB_NONE32;
                         if (bid != CB_NONE32) {
                             const U4 bl = ld16(t.blocks() + bid);
-                            for (uint32_t q = 0; q < bl.y && !deny; q++) {
+                            // (with outputs: (k + 1) passes over the block, pass = the first matching action a row is visited for)
+                            for (uint32_t pq = 0; pq < (Sink::kOn ? (k + 1) * bl.y : bl.y) && !deny; pq++) {
+                                const uint32_t q = Sink::kOn ? pq % bl.y : pq, pass = Sink::kOn ? pq / bl.y : 0;
                                 const uint32_t rix = bl.x + q;
                                 const U4 row = ld16(t.rows() + rix);
                                 if (!kind_has(b, kc, row_respat(row)) || !meta_row_action(b, aset, L->n_rows, ps, kk, rix)) continue;
-                                if (row_drcond(row)) { const uint32_t r = cond_sat(base, L, bp, n, pid, bl.z + row_drcond(row) - 1, cur_edr); unsupported |= r & 2; if (!(r & 1)) continue; }
-                                if (row_cond(row)) { const uint32_t r = cond_sat(base, L, bp, n, pid, bl.z + row_cond(row) - 1, cur_edr); unsupported |= r & 2; if (!(r & 1)) continue; }
+                                if (Sink::kOn && first_action(b, aset, L->n_rows, rix, k) != pass) continue;
+                                if (row_drcond(row)) { const uint32_t r = cond_sat(base, L, bp, n, pid, bl.z + row_drcond(row) - 1, cur_edr); unsupported |= r & 2; if (!(r & 1)) { sink.row(base, L, bp, n, pid, cur_edr, rix, k, false); continue; } }
+                                if (row_cond(row)) { const uint32_t r = cond_sat(base, L, bp, n, pid, bl.z + row_cond(row) - 1, cur_edr); unsupported |= r & 2; if (!(r & 1)) { sink.row(base, L, bp, n, pid, cur_edr, rix, k, false); continue; } }
+                                sink.row(base, L, bp, n, pid, cur_edr, rix, k, true);
                                 if (row_effect(row) == CB_EFFECT_DENY) deny = true; else saw_allow = true;
                             }
                         }
@@ -4471,7 +4599,8 @@ CB_HD_NOINLINE void eval_request_meta(const uint8_t *base, const TableLayout *L,
                                 }
                             }
                             if (deny) break;
-                            for (uint32_t j = 0; j < nk && !deny; j++) {
+                            for (uint32_t pj = 0; pj < (Sink::kOn ? (k + 1) * nk : nk) && !deny; pj++) {
+                                const uint32_t j = Sink::kOn ? pj % nk : pj, pass = Sink::kOn ? pj / nk : 0;
                                 const uint32_t bid = ldg(t.res_block_map() + ((uint64_t)rv * L->nRP + kind_pat_at(b, kc, j)) * L->nS + s);
                                 if (bid == CB_NONE32) continue;
                                 const U4 bl = ld16(t.blocks() + bid);
@@ -4481,8 +4610,10 @@ CB_HD_NOINLINE void eval_request_meta(const uint8_t *base, const TableLayout *L,
                                     const uint32_t rr = row_role(row);
                                     if (!(rr == CB_ROLE_ANY ? a == 0 : (rr == R && in_pr))) continue;
                                     if (!meta_row_action(b, aset, L->n_rows, ps, kk, rix)) continue;
-                                    if (row_drcond(row)) { const uint32_t r = cond_sat(base, L, bp, n, pid, bl.z + row_drcond(row) - 1, cur_edr); unsupported |= r & 2; if (!(r & 1)) continue; }
-                                    if (row_cond(row)) { const uint32_t r = cond_sat(base, L, bp, n, pid, bl.z + row_cond(row) - 1, cur_edr); unsupported |= r & 2; if (!(r & 1)) continue; }
+                                    if (Sink::kOn && first_action(b, aset, L->n_rows, rix, k) != pass) continue;
+                                    if (row_drcond(row)) { const uint32_t r = cond_sat(base, L, bp, n, pid, bl.z + row_drcond(row) - 1, cur_edr); unsupported |= r & 2; if (!(r & 1)) { sink.row(base, L, bp, n, pid, cur_edr, rix, k, false); continue; } }
+                                    if (row_cond(row)) { const uint32_t r = cond_sat(base, L, bp, n, pid, bl.z + row_cond(row) - 1, cur_edr); unsupported |= r & 2; if (!(r & 1)) { sink.row(base, L, bp, n, pid, cur_edr, rix, k, false); continue; } }
+                                    sink.row(base, L, bp, n, pid, cur_edr, rix, k, true);
                                     if (row_effect(row) == CB_EFFECT_DENY) deny = true; else saw_allow = true;
                                 }
                             }
@@ -4511,6 +4642,33 @@ CB_HD_NOINLINE void eval_request_meta(const uint8_t *base, const TableLayout *L,
         atomicOr(status, 1u);
 #else
         *status |= 1u;
+#endif
+    }
+}
+
+CB_HD_NOINLINE void eval_request_meta(const uint8_t *base, const TableLayout *L, const BatchView *bp, uint64_t n, uint8_t *effects, uint32_t *action_meta,
+                                      cb_request_meta *req_meta, uint32_t *status) {
+    NoOutputs none;
+    walk_request(base, L, bp, n, effects, action_meta, req_meta, status, none);
+}
+
+// eval_request_meta's planes plus request n's output record at `rec` (`stride` bytes, 8-byte aligned): every entry or, when
+// they do not fit, none and the size they need.  status: bit 0 a value the device cannot represent, CB_OUT_STATUS_OVERFLOW,
+// CB_OUT_STATUS_UNLOWERED (an entry without a device program was reached).
+CB_HD_NOINLINE void eval_request_outputs(const uint8_t *base, const TableLayout *L, const BatchView *bp, uint64_t n, uint8_t *effects, uint32_t *action_meta,
+                                         cb_request_meta *req_meta, uint32_t *status, uint8_t *rec, uint32_t stride) {
+    OutputSink out; out.rec = rec; out.cap = stride; out.pos = CB_OUT_RECORD_HEADER; out.count = 0; out.status = 0;
+    walk_request(base, L, bp, n, effects, action_meta, req_meta, status, out);
+    const bool fits = out.pos <= stride;
+    cb_out_record *h = reinterpret_cast<cb_out_record *>(rec);
+    h->bytes_needed = out.pos;
+    h->n_entries = fits ? out.count : 0;
+    const uint32_t st = out.status | (fits ? 0u : (uint32_t)CB_OUT_STATUS_OVERFLOW);
+    if (st && status) {
+#if defined(__CUDA_ARCH__)
+        atomicOr(status, st);
+#else
+        *status |= st;
 #endif
     }
 }

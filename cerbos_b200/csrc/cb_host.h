@@ -14,7 +14,7 @@
 
 namespace cbhost {
 
-constexpr int kMaxSec = 32;   // section ids the image carries (cb::TableLayout::off); higher ids are host-only
+constexpr int kMaxSec = CB_IMAGE_SECTIONS;   // section ids the image carries (cb::TableLayout::off); higher ids are host-only
 
 // The checks below report failure as a message ("" = success).
 inline std::string msg(const char *fmt, ...) {

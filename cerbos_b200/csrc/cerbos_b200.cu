@@ -78,6 +78,19 @@ __global__ void __launch_bounds__(kThreads, 2) check_meta_kernel(const __grid_co
     }
 }
 
+// rule-output kernel (cgpu_check_outputs): check_meta_kernel's planes from the same reference-order walk, plus each request's
+// output record, written to the chunk's output slab (record i of the slab: request bv.first + i)
+__global__ void __launch_bounds__(kThreads, 2) check_outputs_kernel(const __grid_constant__ TableDesc td, const __grid_constant__ cb::BatchView bv, uint8_t *effects,
+                                                                uint32_t *action_meta, cb_request_meta *req_meta, uint32_t *status, uint8_t *out_slab,
+                                                                uint32_t stride, uint32_t *needed) {
+    for (uint64_t i = (uint64_t)blockIdx.x * kThreads + threadIdx.x; i < bv.count; i += (uint64_t)gridDim.x * kThreads) {
+        uint8_t *rec = out_slab + i * stride;
+        cb::eval_request_outputs(td.base, &td.lay, &bv, bv.first + i, effects, action_meta, req_meta, status, rec, stride);
+        const uint32_t need = reinterpret_cast<const cb_out_record *>(rec)->bytes_needed;
+        if (need > stride) atomicMax(needed, need);
+    }
+}
+
 // ---- narrow wire format (cgpu_check_narrow): the per-request columns travel over PCIe in their narrowest exact form and are
 // widened to the canonical columns here, in HBM, right before the check kernels read them
 constexpr uint32_t kMaxNarrowSlots = 64;
@@ -1698,7 +1711,16 @@ void cgpu_narrowed_free(cgpu_narrowed *r) {
 struct MetaOut {
     uint32_t *action_meta;          // n_requests * max_actions words
     cb_request_meta *request_meta;  // n_requests records
+    // rule outputs (cgpu_check_outputs; null for the metadata calls): n_requests records of `stride` bytes, and the largest
+    // size a record that did not fit needed (over every device's range)
+    uint8_t *outputs;
+    uint32_t stride;
+    std::atomic<uint32_t> *needed;
 };
+// Device memory of the output records: each stream slot holds two chunk slabs (one filled while the other drains) within
+// this budget, so a call's chunk shrinks as the stride grows instead of device memory growing with stride x chunk.
+static constexpr size_t kOutputSlabBytes = 256ull << 20;
+static constexpr uint32_t kMaxOutputStride = (uint32_t)(kOutputSlabBytes / 2 / 256);   // a chunk keeps at least 256 requests
 
 // requests [lo, hi) of `batch` on ctx's device: pipelined H2D / kernels / D2H (see below); effects_out covers the whole batch.
 // meta: also the metadata plane, from check_meta_kernel in place of the check kernels (nullptr: effects only)
@@ -1784,6 +1806,15 @@ static int check_range(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *bat
         off_am = total; total += ((size_t)N * km * 4 + 255) & ~(size_t)255;
         off_rm = total; total += ((size_t)N * sizeof(cb_request_meta) + 255) & ~(size_t)255;
     }
+    const bool outs = meta && meta->outputs;
+    // output records: two slabs of `chunk` records (chunk below is cut to fit kOutputSlabBytes) and the needed-size word
+    uint64_t out_chunk = 0;
+    size_t off_out = 0, off_need = 0;
+    if (outs) {
+        out_chunk = (kOutputSlabBytes / 2 / meta->stride) & ~(uint64_t)255;
+        off_need = total; total += 256;
+        off_out = total; total += 2 * out_chunk * meta->stride;
+    }
     if (slot->dev_cap < total) {
         if (slot->dev) cudaFree(slot->dev);
         slot->dev = nullptr; slot->dev_cap = 0;
@@ -1819,8 +1850,13 @@ static int check_range(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *bat
     }
     if (chunk < 4096) chunk = 4096;
     chunk &= ~(uint64_t)255;
+    if (outs && chunk > out_chunk) chunk = out_chunk;
     const uint64_t n_chunks = (hi - lo + chunk - 1) / chunk;
-    while (slot->ev.size() < 2 * n_chunks) {
+    const uint64_t n_ev = (outs ? 3 : 2) * n_chunks;   // per chunk: columns in, kernel done, (outputs) output slab drained
+    uint32_t *d_need = reinterpret_cast<uint32_t *>(dbase + off_need);
+    uint8_t *d_out = dbase + off_out;
+    if (outs) CUDA_TRY(cudaMemsetAsync(d_need, 0, 4, slot->stream));
+    while (slot->ev.size() < n_ev) {
         cudaEvent_t e;
         CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
         slot->ev.push_back(e);
@@ -1891,7 +1927,18 @@ static int check_range(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *bat
         cb::BatchView cv = bv;
         cv.first = c0; cv.count = cnt;
         // the kernel writes effect bytes directly (1 ALLOW / 2 DENY / 0 padding): no host post-pass
-        if (meta) {
+        if (outs) {
+            // always the reference-order body: outputs come from the rows it visits, in its order
+            uint8_t *slab = d_out + (k & 1) * out_chunk * meta->stride;
+            if (k >= 2) CUDA_TRY(cudaStreamWaitEvent(slot->stream, slot->ev[2 * n_chunks + k - 2], 0));   // that slab's last copy-out
+            const uint64_t tiles = (cnt + kThreads - 1) / kThreads;
+            const uint32_t grid = (uint32_t)(tiles < (uint64_t)ctx->sm_count * 4 ? tiles : (uint64_t)ctx->sm_count * 4);
+            check_outputs_kernel<<<grid, kThreads, 0, slot->stream>>>(t->desc, cv, d_effects, d_am, d_rm, slot->d_status, slab, meta->stride, d_need);
+            CUDA_TRY(cudaGetLastError());
+            ctx->launches.fetch_add(1, std::memory_order_relaxed);
+            ctx->last_plan = LaunchPlan();
+            ctx->last_grid = grid;
+        } else if (meta) {
             // the unique-condition kernel the effect launch would run, in its metadata form, where the table has the side
             // table that form reads; else the reference-order body for every request
             const LaunchPlan plan = plan_launch(*ctx, *t, cv);
@@ -1919,13 +1966,28 @@ static int check_range(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *bat
             CUDA_TRY(cudaMemcpyAsync(meta->action_meta + c0 * km, d_am + c0 * km, cnt * km * 4, cudaMemcpyDeviceToHost, slot->d2h));
             CUDA_TRY(cudaMemcpyAsync(meta->request_meta + c0, d_rm + c0, cnt * sizeof(cb_request_meta), cudaMemcpyDeviceToHost, slot->d2h));
         }
+        if (outs) {
+            const uint8_t *slab = d_out + (k & 1) * out_chunk * meta->stride;
+            CUDA_TRY(cudaMemcpyAsync(meta->outputs + c0 * meta->stride, slab, cnt * meta->stride, cudaMemcpyDeviceToHost, slot->d2h));
+            CUDA_TRY(cudaEventRecord(slot->ev[2 * n_chunks + k], slot->d2h));
+        }
     }
+    uint32_t h_need = 0;
+    if (outs) CUDA_TRY(cudaMemcpyAsync(&h_need, d_need, 4, cudaMemcpyDeviceToHost, slot->d2h));
     CUDA_TRY(cudaMemcpyAsync(slot->h_status, slot->d_status, 4, cudaMemcpyDeviceToHost, slot->d2h));   // behind the last chunk's results
     CUDA_TRY(cudaStreamSynchronize(slot->d2h));
     quiesce.armed = false;   // d2h waited for every kernel, every kernel for its columns: all three streams are idle
-    if (*slot->h_status) {
+    if (const uint32_t st = *slot->h_status) {
         CUDA_TRY(cudaMemset(slot->d_status, 0, 4));
-        return fail(CGPU_ERR_UNSUPPORTED, "a request produced a run-time value the device cannot represent exactly (e.g. timestamp outside 1678..2262, string->double, concatenation)");
+        if (st & 1u)
+            return fail(CGPU_ERR_UNSUPPORTED, "a request produced a run-time value the device cannot represent exactly (e.g. timestamp outside 1678..2262, string->double, concatenation)");
+        if (outs && (st & cb::CB_OUT_STATUS_UNLOWERED))
+            return fail(CGPU_ERR_UNSUPPORTED, "a request reached a rule output the device cannot evaluate (the table's MANIFEST lists them as unlowered_outputs)");
+        if (outs && (st & cb::CB_OUT_STATUS_OVERFLOW)) {
+            uint32_t cur = meta->needed->load();
+            while (h_need > cur && !meta->needed->compare_exchange_weak(cur, h_need)) {}
+            return fail(CGPU_ERR_UNSUPPORTED, "rule outputs: a request's output record needs %u bytes, more than the stride of %u", h_need, meta->stride);
+        }
     }
     return CGPU_OK;
 }
@@ -1986,6 +2048,21 @@ int cgpu_check_meta(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch,
     if (t->ctx != ctx) return fail(CGPU_ERR_INVALID, "table belongs to another context");
     const MetaOut meta{action_meta_out, static_cast<cb_request_meta *>(request_meta_out)};
     return check_sharded(ctx, t, batch, effects_out, nullptr, &meta);
+}
+
+int cgpu_check_outputs(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch, uint8_t *effects_out, uint32_t *action_meta_out,
+                       void *request_meta_out, uint8_t *outputs_out, uint32_t outputs_stride, uint32_t *outputs_bytes_needed) {
+    if (!ctx || !t || !batch || !effects_out || !action_meta_out || !request_meta_out || !outputs_out || !outputs_bytes_needed)
+        return fail(CGPU_ERR_INVALID, "cgpu_check_outputs: null argument");
+    if (t->ctx != ctx) return fail(CGPU_ERR_INVALID, "table belongs to another context");
+    *outputs_bytes_needed = 0;
+    if (outputs_stride < CB_OUT_RECORD_HEADER || outputs_stride % 8 || outputs_stride > kMaxOutputStride)
+        return fail(CGPU_ERR_INVALID, "cgpu_check_outputs: outputs_stride %u (a multiple of 8 in [%d, %u])", outputs_stride, CB_OUT_RECORD_HEADER, kMaxOutputStride);
+    std::atomic<uint32_t> needed{0};
+    const MetaOut meta{action_meta_out, static_cast<cb_request_meta *>(request_meta_out), outputs_out, outputs_stride, &needed};
+    const int rc = check_sharded(ctx, t, batch, effects_out, nullptr, &meta);
+    *outputs_bytes_needed = needed.load();
+    return rc;
 }
 
 int cgpu_check_narrow_meta(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch, const cgpu_narrow *narrow, uint8_t *effects_out,

@@ -10,7 +10,10 @@ an input appears in its output with EFFECT_ALLOW or EFFECT_DENY; any failure rai
 
 ``check(..., include_meta=True)`` also fills ``policy`` / ``scope`` of every action and ``effectiveDerivedRoles`` (the
 reference's IncludeMeta responses, cerbos_svc.go:291-311) from the device's metadata plane (cgpu_check_meta).
-Not produced (SURVEY.md 8(f)): rule outputs, validation errors, audit trail.
+``check(..., include_outputs=True)`` also fills ``outputs`` of every input: the rule outputs (ruletable.go:1065-1106) in the
+reference's emission order, from the device (cgpu_check_outputs), with the metadata of include_meta.  ``has_outputs`` tells
+whether the table declares any; ``unlowered_outputs`` lists those the device cannot evaluate (a request reaching one fails).
+Not produced (SURVEY.md 8(f)): validation errors, audit trail.
 """
 from __future__ import annotations
 
@@ -68,6 +71,15 @@ class Engine:
         if old is not None:
             old.release()
 
+    @property
+    def has_outputs(self) -> bool:
+        return bool(self.flat.manifest.get("output_sources"))
+
+    @property
+    def unlowered_outputs(self) -> list:
+        """[{"policy", "rule", "kind", "when", "reason"}]: outputs without a device program."""
+        return list(self.flat.manifest.get("unlowered_outputs") or [])
+
     def check_effects(self, inputs, now_ns=None):
         """-> (Batch, uint8[n, K] effects)"""
         if now_ns is None:
@@ -77,13 +89,14 @@ class Engine:
         eff = self.table.check(batch.columns, batch.n, batch.max_actions, now_ns, flags)
         return batch, eff
 
-    def check(self, inputs, now_ns=None, include_meta=False):
+    def check(self, inputs, now_ns=None, include_meta=False, include_outputs=False):
         """-> list of CheckOutput dicts, index-aligned with `inputs`.  include_meta: also `policy` / `scope` per action
-        and `effectiveDerivedRoles` (ruletable.go:753-782), through the metadata plane of the device."""
+        and `effectiveDerivedRoles` (ruletable.go:753-782), through the metadata plane of the device.  include_outputs:
+        that, and `outputs` ([{"src", "action", "val"}] in emission order)."""
         if not inputs:
             return []
-        if include_meta:
-            return self._check_with_meta(inputs, now_ns)
+        if include_meta or include_outputs:
+            return self._check_with_meta(inputs, now_ns, include_outputs)
         batch, eff = self.check_effects(inputs, now_ns)
         outs = []
         for i, inp in enumerate(inputs):
@@ -94,14 +107,29 @@ class Engine:
                          "actions": actions})
         return outs
 
-    def _check_with_meta(self, inputs, now_ns=None):
+    OUTPUT_STRIDE = 4096   # first guess of an output record's size; a call whose records need more is repeated once with that
+
+    def _check_with_meta(self, inputs, now_ns=None, include_outputs=False):
         from . import meta as M
         if now_ns is None:
             now_ns = time.time_ns()
         batch = self.encoder.encode(inputs)
         flags = L.BATCH_FLAG_LENIENT if self.conf["lenient_scope_search"] else 0
-        eff, am, rm = self.table.check_meta(batch.columns, batch.n, batch.max_actions, now_ns, flags)
         man = self.flat.manifest
+        entries = None
+        if include_outputs:
+            from . import outputs as O
+            stride = self.OUTPUT_STRIDE
+            try:
+                eff, am, rm, rec, _ = self.table.check_outputs(batch.columns, batch.n, batch.max_actions, stride, now_ns, flags)
+            except capi.CgpuError as e:
+                if not getattr(e, "bytes_needed", 0):
+                    raise
+                stride = (e.bytes_needed + 7) // 8 * 8
+                eff, am, rm, rec, _ = self.table.check_outputs(batch.columns, batch.n, batch.max_actions, stride, now_ns, flags)
+            entries = O.decode(rec, stride, man, [inp.get("actions") or [] for inp in inputs])
+        else:
+            eff, am, rm = self.table.check_meta(batch.columns, batch.n, batch.max_actions, now_ns, flags)
         outs = []
         for i, inp in enumerate(inputs):
             p, r = inp.get("principal") or {}, inp.get("resource") or {}
@@ -113,6 +141,8 @@ class Engine:
                 actions[a] = {"effect": EFFECT_NAMES[int(eff[i, k])], "policy": policy, "scope": scope}
             outs.append({"requestId": inp.get("requestId", ""), "resourceId": r.get("id", ""), "actions": actions,
                          "effectiveDerivedRoles": M.decode_edr(int(rm[i]["effective_derived_roles"]), man)})
+            if entries is not None:
+                outs[-1]["outputs"] = entries[i]
         return outs
 
     def close(self):

@@ -284,14 +284,15 @@ class ProgramCompiler:
         self.sp = 0
         self.loop_vars: list[dict] = []   # stack of {name: var index}
         self.inlining: list[str] = []
+        self.stack_limit = L.MAX_STACK    # value programs (rule outputs) run with the deeper OUT_MAX_STACK
 
     # ---------------------------------------------------------------- emit helpers
     def emit(self, op, a=0, b=0, c=0, delta=0):
         self.code.append([OP[op], a, b, c])
         self.sp += delta
-        if self.sp > self.ctx.max_stack:
+        if self.sp > self.ctx.max_stack and self.stack_limit == L.MAX_STACK:
             self.ctx.max_stack = self.sp
-        if self.sp > L.MAX_STACK:
+        if self.sp > self.stack_limit:
             raise Unsupported("expression needs a deeper evaluation stack than the device provides")
         return len(self.code) - 1
 
@@ -1402,5 +1403,14 @@ def compile_condition(ctx: TableBuilderCtx, cond: Cond, params: Params | None) -
     """Condition tree -> instruction list [[op, a, b, c], ...] leaving a plain BOOL."""
     pc = ProgramCompiler(ctx, params)
     pc.compile_cond(cond)
+    assert pc.sp == 1, pc.sp
+    return pc.finish()
+
+
+def compile_value(ctx: TableBuilderCtx, expr, params: Params | None) -> list:
+    """Expression -> instruction list leaving its VALUE (a rule output): the condition compiler's path without TO_COND."""
+    pc = ProgramCompiler(ctx, params)
+    pc.stack_limit = L.OUT_MAX_STACK
+    pc.expr(expr.ast)
     assert pc.sp == 1, pc.sp
     return pc.finish()

@@ -30,7 +30,7 @@ from ..policy import namer
 from ..policy.globs import is_glob
 from ..policy.model import KIND_PRINCIPAL, KIND_RESOURCE, RuleTable, SP_UNSPECIFIED
 from . import layout as L
-from .bytecode import TableBuilderCtx, Unsupported, compile_condition, compile_flat, const_v64
+from .bytecode import TableBuilderCtx, Unsupported, compile_condition, compile_flat, compile_value, const_v64
 
 
 class _Dict:
@@ -154,6 +154,7 @@ def flatten(rt: RuleTable, globals_=None) -> FlatTable:
             groups[key].append(r)
 
     blocks, row_recs, conds, code, row_apats = [], [], [], [], []
+    pending_outputs: list = []   # (row index, Row) of every row with a rule output, compiled after all conditions
     dr_off, dr_entries, dr_parents = [], [], []
     block_shapes: set = set()
     code_ix: dict[tuple, tuple] = {}
@@ -213,8 +214,12 @@ def flatten(rt: RuleTable, globals_=None) -> FlatTable:
             return li
 
         row_start = len(row_recs)
-        # rows that differ only in their action pattern are merged into one row with a pattern list
+        # rows that differ only in their action pattern are merged into one row with a pattern list -- except in a block
+        # with rule outputs, where every rule action stays a row of its own in the reference's order: outputs are emitted
+        # per visited row, and a merged row could move a DENY ahead of an output row
+        with_outputs = any(r.emit_activated is not None or r.emit_not_met is not None for r in grows)
         merged: dict[tuple, list] = {}
+        out_rows: list = []
         for r in grows:
             try:
                 c_ix, dc_ix = local_cond(r.condition, r.params), local_cond(r.dr_condition, r.dr_params)
@@ -228,18 +233,24 @@ def flatten(rt: RuleTable, globals_=None) -> FlatTable:
             key2 = (L.ROLE_ANY if r.role == "*" else roles.ids[r.role], c_ix, dc_ix,
                     respats.ids[r.resource] if kind == "P" else L.NONE16, r.effect,
                     L.ROW_FLAG_PRINCIPAL if kind == "P" else 0)
-            pats = merged.setdefault(key2, [])
             ap = apats.ids[r.action]
+            if with_outputs:
+                out_rows.append((key2, [ap]))
+                if r.emit_activated is not None or r.emit_not_met is not None:
+                    pending_outputs.append((row_start + len(out_rows) - 1, r))
+                continue
+            pats = merged.setdefault(key2, [])
             if ap not in pats:
                 pats.append(ap)
-        for key2, pats in merged.items():
+        block_rows = out_rows if with_outputs else list(merged.items())
+        for key2, pats in block_rows:
             if len(pats) > 0xFFFF:
                 raise Unsupported("too many action patterns on one rule")
             row_recs.append(key2 + (len(pats), len(row_apats)))
             row_apats.extend(pats)
         blocks.append((row_start, len(row_recs) - row_start, cond_base, len(conds) - cond_base))
         # shape of the block = everything that steers the kernel's control flow through it
-        block_shapes.add((tuple(k2[:3] + k2[4:] + (tuple(p),) for k2, p in merged.items()), tuple(conds[cond_base:])))
+        block_shapes.add((tuple(k2[:3] + k2[4:] + (tuple(p),) for k2, p in block_rows), tuple(conds[cond_base:])))
         # derived roles of this resource policy (evaluated once per scope for effectiveDerivedRoles, ruletable.go:936-979);
         # the reference looks them up under the request's own kind, so only exact-name policies carry any
         dr_off.append(len(dr_entries))
@@ -296,6 +307,41 @@ def flatten(rt: RuleTable, globals_=None) -> FlatTable:
                     par_list.extend(roles.ids[p] for p in acc)
         par_off[nS * nR] = len(par_list)
 
+    # ---- rule outputs (after every condition, so that a table's slots, constants and code offsets keep their numbers) -----
+    # An expression the device cannot lower leaves its entry unlowered: the table still builds, and only a request that
+    # visits the row fails (CGPU_ERR_UNSUPPORTED).
+    row_out = np.full(max(len(row_recs), 1), L.NONE32, dtype=np.uint32)
+    out_entries, out_srcs, unlowered = [], _Dict(), []
+
+    def add_output(expr, params):
+        try:
+            prog = compile_value(ctx, expr, params)
+        except Unsupported as e:
+            return None, str(e)
+        ent = code_ix.get(tuple(tuple(i) for i in prog))
+        if ent is None:
+            ent = (len(code), len(prog))
+            code_ix[tuple(tuple(i) for i in prog)] = ent
+            code.extend(prog)
+        return ent[0], ""
+
+    for rix, r in pending_outputs:
+        src = f"{namer.policy_key_from_fqn(r.origin_fqn)}#{r.name}"
+        offs, flags = [L.NONE32, L.NONE32], 0
+        for w, (expr, bit, when) in enumerate(((r.emit_activated, L.OUT_UNLOWERED_ACTIVATED, "ruleActivated"),
+                                              (r.emit_not_met, L.OUT_UNLOWERED_NOT_MET, "conditionNotMet"))):
+            if expr is None:
+                continue
+            off, why = add_output(expr, r.params)
+            if off is None:
+                flags |= bit
+                unlowered.append({"policy": namer.policy_key_from_fqn(r.origin_fqn), "rule": r.name, "kind": r.resource,
+                                  "when": when, "reason": why})
+            else:
+                offs[w] = off
+        row_out[rix] = len(out_entries)
+        out_entries.append((out_srcs.add(src), offs[0], offs[1], flags))
+
     # ---- strings: everything the kernels may compare against request strings ---------------------------------------
     # principals must be table strings so that hdr.principal_id (a string id) can be mapped to a principal index
     prin_str = [ctx.strings.intern(p) for p in principals.items]
@@ -325,7 +371,8 @@ def flatten(rt: RuleTable, globals_=None) -> FlatTable:
         max_loop_depth=ctx.max_loop_depth, n_vars=ctx.n_vars, theap_words=len(ctx.theap),
         uses_pid=int(ctx.uses_pid), uses_now=int(ctx.uses_now), max_scope_depth=max_depth,
         direct_kinds=int(not any(is_glob(p) for p in respats.items)), block_shapes=len(block_shapes),
-        uses_runtime=int(ctx.uses_runtime), n_dr_names=len(dr_names),
+        uses_runtime=int(ctx.uses_runtime), n_dr_names=len(dr_names), n_output_rows=len(out_entries),
+        n_unlowered_outputs=len(unlowered),
     ).items():
         meta[L.META[k]] = val
 
@@ -387,6 +434,9 @@ def flatten(rt: RuleTable, globals_=None) -> FlatTable:
         "row_pat_start": [int(r[7]) for r in row_recs], "row_apats": [int(x) for x in row_apats],
         "derived_roles": dr_names,
     }
+    if out_entries:
+        manifest["output_sources"] = out_srcs.items
+        manifest["unlowered_outputs"] = unlowered
     man_bytes = json.dumps(manifest, ensure_ascii=False, separators=(",", ":")).encode("utf-8")
 
     secs = [
@@ -408,8 +458,10 @@ def flatten(rt: RuleTable, globals_=None) -> FlatTable:
         ("DR_ENTRIES", np.array(dr_entries or [(0, 0, 0, 0)], dtype=np.uint32).reshape(-1, 4), 16),
         ("DR_PARENTS", np.array(dr_parents or [0], dtype=np.uint32), 4),
         ("DR_NAME_STR", np.array(dr_name_str or [0], dtype=np.uint32), 4),
-        ("MANIFEST", np.frombuffer(man_bytes, dtype=np.uint8), 1),
     ]
+    if out_entries:
+        secs += [("ROW_OUT", row_out, 4), ("OUT_ENTRIES", np.array(out_entries, dtype=np.uint32).reshape(-1, 4), 16)]
+    secs.append(("MANIFEST", np.frombuffer(man_bytes, dtype=np.uint8), 1))
     assert rows_a.dtype.itemsize == 16 and code_a.dtype.itemsize == 8 and consts_a.dtype.itemsize == 16
 
     hdr_bytes = 32 + 24 * len(secs)

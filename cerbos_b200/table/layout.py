@@ -12,7 +12,7 @@ Table blob (little endian, every section 16-byte aligned):
 from __future__ import annotations
 
 MAGIC = 0x32425243  # 'CRB2'
-VERSION = 16
+VERSION = 17
 ALIGN = 16
 
 NONE32 = 0xFFFFFFFF
@@ -58,6 +58,9 @@ SECTIONS = {
     "DR_ENTRIES": 28,     # {u32 name index (MANIFEST derived_roles, sorted); cond (global id + 1, 0 none); parents start; n parents}
     "DR_PARENTS": 29,     # u32[] parent role ids (ROLE_ANY for "*")
     "DR_NAME_STR": 30,    # u32[n derived role names] string id of each name (runtime.effectiveDerivedRoles in conditions)
+    # rule outputs (present only when the table declares outputs; blocks holding an output row keep one row per rule action)
+    "ROW_OUT": 31,        # u32[n_rows] OUT_ENTRIES index of the row | NONE32
+    "OUT_ENTRIES": 32,    # {u32 src id (MANIFEST output_sources); activated code_off | NONE32; not-met code_off | NONE32; flags OUT_UNLOWERED_*}
     "MANIFEST": 100,      # JSON (host only): dictionaries + slot paths for the batch encoder
 }
 
@@ -66,8 +69,9 @@ META = {name: i for i, name in enumerate([
     "n_versions", "n_respats", "n_scopes", "n_principals", "n_roles", "n_apats", "n_blocks", "n_rows",
     "n_conds", "n_code", "n_consts", "n_slots", "n_strings", "has_role_policies", "has_parent_roles",
     "has_principal_policies", "max_stack", "max_loop_depth", "n_vars", "theap_words", "uses_pid", "uses_now",
-    "max_scope_depth", "direct_kinds", "block_shapes", "uses_runtime", "n_dr_names",
+    "max_scope_depth", "direct_kinds", "block_shapes", "uses_runtime", "n_dr_names", "n_output_rows", "n_unlowered_outputs",
 ])}
+IMAGE_SECTIONS = 33   # section ids below this travel in the device image (TableLayout::off); MANIFEST is host-only
 
 SCOPE_FLAG_PRINCIPAL = 1
 SCOPE_FLAG_RESOURCE = 2
@@ -231,6 +235,24 @@ MAX_CLASS_PATS = 8  # resource patterns one request kind may match
 # decision metadata: where ActionEffect.Policy comes from (ruletable.go:913-922, 1082-1095)
 META_SRC = {"NO_MATCH": 0, "PRINCIPAL_POLICY": 1, "RESOURCE_POLICY": 2, "NO_MATCH_FOR_SCOPE_PERMISSIONS": 3, "ROLE_POLICY": 4}
 
+# rule outputs (cgpu_check_outputs).  OUT_ENTRIES.flags: the activated / not-met expression has no device program; a
+# request that visits it fails the call with CGPU_ERR_UNSUPPORTED.
+OUT_UNLOWERED_ACTIVATED = 1
+OUT_UNLOWERED_NOT_MET = 2
+# Output records: every request owns `stride` bytes {u32 bytes_needed; u32 n_entries} + entries in emission order.  An entry
+# is {u16 action index; u16 pad; u32 src id} + one value; a value is a tag byte + payload (little endian, unaligned):
+#   BOOL u8 | INT i64 | UINT u64 | DOUBLE f64 | STRING / BYTES u32 length + bytes | TIMESTAMP / DURATION i64 nanoseconds |
+#   LIST u32 n + n values | MAP u32 n + n (key, value) pairs | NO_VALUE (evaluation error), NULL, NOT_CONVERTIBLE: nothing.
+# Values are CEL-typed; the conversion to google.protobuf.Value happens on the host (cerbos_b200/outputs.py).
+OUT_TAGS = {name: i for i, name in enumerate([
+    "NO_VALUE", "NULL", "BOOL", "INT", "UINT", "DOUBLE", "STRING", "BYTES", "TIMESTAMP", "DURATION", "LIST", "MAP",
+    "NOT_CONVERTIBLE",
+])}
+OUT_RECORD_HEADER = 8
+OUT_ENTRY_HEADER = 8
+OUT_MAX_STACK = 32  # evaluation stack of a value program (literal maps and lists of a rule output sit on it whole)
+OUT_MAX_DEPTH = 8   # nesting of lists / maps an output value may have on the device (deeper: CGPU_ERR_UNSUPPORTED)
+
 # batch flags (cgpu_batch.flags)
 BATCH_FLAG_LENIENT = 1
 
@@ -323,6 +345,15 @@ def c_header() -> str:
     d("CB_FMT_PREC_DEFAULT", FMT_PREC_DEFAULT, True)
     for k, v in META_SRC.items():
         d(f"CB_META_SRC_{k}", v)
+    d("CB_IMAGE_SECTIONS", IMAGE_SECTIONS)
+    d("CB_OUT_UNLOWERED_ACTIVATED", OUT_UNLOWERED_ACTIVATED)
+    d("CB_OUT_UNLOWERED_NOT_MET", OUT_UNLOWERED_NOT_MET)
+    for k, v in OUT_TAGS.items():
+        d(f"CB_OUT_{k}", v)
+    d("CB_OUT_RECORD_HEADER", OUT_RECORD_HEADER)
+    d("CB_OUT_ENTRY_HEADER", OUT_ENTRY_HEADER)
+    d("CB_OUT_MAX_STACK", OUT_MAX_STACK)
+    d("CB_OUT_MAX_DEPTH", OUT_MAX_DEPTH)
     out.append("")
     out.append("""typedef struct { uint32_t magic, version, n_sections, flags; uint64_t total_bytes, reserved; } cb_blob_header;
 typedef struct { uint32_t id, elem_bytes; uint64_t offset, n_bytes; } cb_section_desc;
@@ -338,6 +369,9 @@ typedef struct { uint32_t respat, cond, apat_start, n_apats; } cb_rolepol_rule;
  * source << 16 | role id << 24 (source CB_META_SRC_ROLE_POLICY) -- and per request the first scope of each chain + the
  * effective derived roles as a bit set over MANIFEST.derived_roles */
 typedef struct { uint16_t principal_first_scope, resource_first_scope; uint32_t flags; uint64_t effective_derived_roles; } cb_request_meta;
+/* rule outputs (cgpu_check_outputs): an OUT_ENTRIES record, and the head of every request's output record */
+typedef struct { uint32_t src, activated, not_met, flags; } cb_out_entry;
+typedef struct { uint32_t bytes_needed, n_entries; } cb_out_record;
 /* request header columns (SURVEY.md 8(d): 24 B / request) */
 typedef struct { uint32_t principal_id, kind_class, resource_scope, principal_scope; } cb_hdr0;   /* 16 B */
 typedef struct { uint16_t resource_version, principal_version; uint32_t action_set_id; } cb_hdr1;  /*  8 B */

@@ -193,6 +193,20 @@ int cgpu_check_meta(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch,
  * loop order, one action after another, so a call takes 25-50x as long as cgpu_check_narrow (DESIGN.md section 7). */
 int cgpu_check_narrow_meta(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch, const cgpu_narrow *narrow, uint8_t *effects_out,
                            uint32_t *action_meta_out, void *request_meta_out /* cb_request_meta[n_requests] */);
+/* Rule outputs (RuleRow.emit_output, ruletable.go:1065-1106): cgpu_check_meta's three outputs plus, for every request, the
+ * output entries of the rows the reference's walk visits, in its order -- together a whole CheckOutput.  Inputs as cgpu_check.
+ *   outputs_out           n_requests records of outputs_stride bytes (a multiple of 8, at least 8): {u32 bytes_needed;
+ *                         u32 n_entries} then the entries, each {u16 action index; u16 pad; u32 src id (MANIFEST
+ *                         output_sources)} and one CEL-typed value (CB_OUT_* tags, cerbos_b200_format.h; decoded and
+ *                         converted to google.protobuf.Value by the host, cerbos_b200/outputs.py)
+ *   outputs_bytes_needed  the largest bytes_needed of a record that did not fit its stride, else 0
+ * Fails with CGPU_ERR_UNSUPPORTED when a record does not fit (it then holds no entries; retry with the size reported), when
+ * a request reaches an output the table build could not lower (table META n_unlowered_outputs, MANIFEST unlowered_outputs),
+ * or on a value the device cannot represent.  Runs the reference-order body on cgpu_check's pipeline and devices; device
+ * memory for the records is bounded per stream slot, so large strides take smaller chunks. */
+int cgpu_check_outputs(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch, uint8_t *effects_out, uint32_t *action_meta_out,
+                       void *request_meta_out /* cb_request_meta[n_requests] */, uint8_t *outputs_out, uint32_t outputs_stride,
+                       uint32_t *outputs_bytes_needed);
 
 /* Device-resident path: columns are device pointers on ctx's device.  dev_bitmap_out receives
  * n_requests * ceil(max_actions / 8) bytes, bit (k % 8) of byte n * ceil(K/8) + k / 8 set <=> ALLOW.

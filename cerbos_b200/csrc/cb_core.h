@@ -3881,6 +3881,17 @@ CB_HD ListRegs list_load(const TableView t, const BatchView &b, uint64_t x) {
     if (L.st == 0) L.st = odd ? 2u : 0u;
     return L;
 }
+// List-header prefetch (cb_kernels.h: check_uc_body).  While a warp finishes its chunk, each lane pulls towards L2 the
+// header line of every list its next request will list_load, so that the header round of that load finds it there.
+// The encoder writes a batch's lists request after request, one heap region per slot: the headers of 32 consecutive
+// requests cover the few 128-byte lines that also hold their elements.  Only batch-heap lists count: table-heap lists
+// are constants that stay L2-resident.  nullptr: nothing to prefetch (absent, error, another type, a table-heap list, or
+// an offset at or past the end of the heap); any other result is a word of [b.heap, b.heap + b.heap_words).
+CB_HD const uint64_t *list_header_pf(const BatchView &b, uint64_t x) {
+    if (v64_tag(x) != CB_V64_LIST || !(x & CB_V64_HEAP_BATCH_BIT)) return nullptr;
+    const uint64_t off = x & (CB_V64_HEAP_BATCH_BIT - 1);
+    return off < b.heap_words ? b.heap + off : nullptr;
+}
 // size(x) / x[i] from the list registers L = list_load(x): the SLOT_SIZE / SLOT_ELEM operands of term_operand() for
 // every value.  The length is the list header (exact for st 0 and 2); an element is in registers only for st 0.
 CB_HD uint64_t list_size(const TableView t, const BatchView &b, uint64_t x, const ListRegs &L) {
@@ -4893,6 +4904,7 @@ constexpr uint32_t kUcRowsOfLayout = ~0u;   // Conds::kDenyRows / kAllowRows of 
 struct GenericConds {
     static constexpr int kForm = CB_UC_FORM_MASK64;   // the condition word may use all 64 bits
     static constexpr uint32_t kDenyRows = kUcRowsOfLayout, kAllowRows = kUcRowsOfLayout;   // the image's form is read at run time
+    static constexpr uint32_t kListSlots = 0;   // no register-resident lists: no heap prefetch (cb_kernels.h: check_uc_body)
     template <typename Cols>
     CB_HD Cols load(const TableView, const BatchView &, const Cols &cols) const { return cols; }
     template <typename Cols>

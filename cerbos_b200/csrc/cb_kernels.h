@@ -379,6 +379,20 @@ __device__ __forceinline__ void check_uc_body(const TableDesc &td, const cb::Bat
                 bv.defer_list[k] = (uint32_t)i;
             }
         }
+#ifndef CB_UC_NO_LIST_PF   // tools/uc_variants.sh: without the list-header prefetch
+        if constexpr (Conds::kListSlots > 0) {
+            // this warp's next chunk: pull the headers of its register-resident lists towards L2 (cb::list_header_pf).
+            // Here, after the walk, the next chunk's slot words are L2 hits (prefetched above, one chunk ago) and hold
+            // no register during the term evaluation.  Prefetches never fault and change no value.
+            const uint64_t i2 = (chunk + n_warps) * 32 + lane;
+            if (i2 < bv.count) {
+#pragma unroll
+                for (uint32_t s = 0; s < Conds::kListSlots; s++)
+                    if (const uint64_t *p = cb::list_header_pf(bv, cb::ldcol64(bv.slots + (uint64_t)Conds::kListSlot[s] * bv.stride + bv.first + i2)))
+                        asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
+            }
+        }
+#endif
     }
 }
 

@@ -804,6 +804,15 @@ inline UcSource generate_uc(const uint8_t *uc_image, const uint32_t *off, uint32
     s += "    static constexpr uint32_t kDenyRows = " + std::to_string(deny_rows) + "u, kAllowRows = " + std::to_string(allow_rows) +
          "u;   // segment slots (0 / 0: row ranges)\n";
     s += std::string("    static constexpr bool kPrograms = ") + (have_atoms ? "true" : "false") + ";   // leaf programs: needs the value helpers of cb_core.h\n";
+    {   // the slots load() keeps as register-resident lists: the kernel prefetches their headers a chunk ahead.  Not for
+        // tables with leaf programs (2 CTAs / SM and a stack frame): on C5 the prefetch made the kernel slower (DESIGN §7)
+        std::string ls;
+        uint32_t nls = 0;
+        for (uint32_t v = 0; v < ns && !have_atoms; v++)
+            if (slot_list[v]) ls += (nls++ ? ", " : "") + std::to_string(v) + "u";
+        s += "    static constexpr uint32_t kListSlots = " + std::to_string(nls) + "u;   // list slots whose headers check_uc_body prefetches\n";
+        s += "    static constexpr uint32_t kListSlot[" + std::to_string(nls ? nls : 1u) + "] = {" + (nls ? ls : "0u") + "};\n";
+    }
     s += "    template <typename Cols>\n    CB_HD SpecRegs load(const TableView t, const BatchView &b, const Cols &c) const {\n        SpecRegs r;\n        r.g.b = c.b; r.g.n = c.n;\n";
     for (uint32_t v = 0; v < ns; v++)
         if (reg(v)) s += "        r.s" + std::to_string(v) + " = c.slot(" + std::to_string(v) + "u);\n";

@@ -5,6 +5,7 @@
 # (cb_core.h: CB_UC_STUB_*; their decisions are wrong, hence --no-verify): default minus stub = that phase's share.
 # stub_lists drops the list loads and compares, stub_list_probes only the compares (list_probe, list_mask).
 # stub_fallback keeps only the typed branch of a table that has one (the path a request of well-typed attributes runs).
+# no_list_pf drops the prefetch of the next chunk's list headers (cb_kernels.h: check_uc_body; results unchanged).
 OUT=${OUT:-profile_out}; mkdir -p "$OUT"
 N=${1:-16777216}
 out=$OUT/uc_variants.txt
@@ -21,6 +22,7 @@ run stub_list_probes CERBOS_B200_SPEC_DEFS=-DCB_UC_STUB_LIST_PROBES
 run stub_strpred CERBOS_B200_SPEC_DEFS=-DCB_UC_STUB_STRPRED
 run stub_fallback CERBOS_B200_SPEC_DEFS=-DCB_UC_STUB_FALLBACK
 run stub_terms CERBOS_B200_SPEC_DEFS=-DCB_UC_STUB_TERMS
+run no_list_pf CERBOS_B200_SPEC_DEFS=-DCB_UC_NO_LIST_PF
 run keys64 CERBOS_B200_SPEC_DEFS=-DCB_LIST_KEYS64
 run blocks3 CERBOS_B200_SPEC_UC_BLOCKS=3
 run blocks4 CERBOS_B200_SPEC_UC_BLOCKS=4

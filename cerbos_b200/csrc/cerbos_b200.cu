@@ -200,6 +200,80 @@ __global__ void __launch_bounds__(kThreads) widen_heap16_kernel(const uint16_t *
     }
 }
 
+// ------------------------------------------------------------------------------------------- host side: errors, narrow wire
+thread_local std::string g_err;
+
+int fail(int code, const char *fmt, ...) {
+    char buf[512];
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(buf, sizeof(buf), fmt, ap);
+    va_end(ap);
+    g_err = buf;
+    return code;
+}
+#define CUDA_TRY(expr)                                                                                   \
+    do {                                                                                                 \
+        cudaError_t e__ = (expr);                                                                        \
+        if (e__ != cudaSuccess) return fail(CGPU_ERR_CUDA, "%s failed: %s", #expr, cudaGetErrorString(e__)); \
+    } while (0)
+
+// The narrow wire on the host (a descriptor narrow_args accepted): the columns are staged in the slot's device buffer
+constexpr uint8_t kNarrowElemBytes[] = {8, 4, 4, 4, 1, 2, 1};   // bytes per request of a slot column, by CGPU_SLOT_* class
+inline uint32_t narrow_hdr_w(const cgpu_narrow &nb) { return 4u - (uint32_t)__builtin_popcount(nb.hdr_const_mask & 15u); }   // header fields that travel
+
+// Byte offsets of one call's data in its slot's device buffer (slot_layout), in this order, each region rounded up to 256
+// bytes; a region the call does not use is empty (offset 0 behind the effect bytes)
+struct SlotLayout {
+    size_t col[CGPU_N_COLUMNS], effects;                                           // the canonical columns, the effect bytes
+    struct { size_t pid, hdr16, versions, roles, slot[kMaxNarrowSlots], heap; } narrow;   // a narrow batch's columns as they travel
+    size_t action_meta, request_meta;                                             // the metadata planes
+    size_t needed, out; uint64_t out_chunk;   // rule outputs: the needed-size word, two slabs of out_chunk records
+    size_t total;
+};
+
+// The widening parameters of one call but its chunk (first / count), over the slot's device buffer `dev`, columns of stride N
+WidenParams widen_params(const cgpu_narrow &nb, uint64_t N, uint32_t n_slots, uint8_t *dev, const SlotLayout &L) {
+    WidenParams wp{};
+    wp.pid = reinterpret_cast<const uint32_t *>(dev + L.narrow.pid); wp.pid16 = nb.principal_id16 ? reinterpret_cast<const uint16_t *>(dev + L.narrow.pid) : nullptr;
+    wp.pid_base = nb.principal_base; wp.hdr16 = reinterpret_cast<const uint16_t *>(dev + L.narrow.hdr16);
+    wp.hdr_const_mask = nb.hdr_const_mask; wp.hdr_w = narrow_hdr_w(nb);
+    for (int f = 0; f < 4; f++) wp.hdr_const[f] = nb.hdr_const[f];
+    wp.versions = dev + L.narrow.versions; wp.versions_const = nb.versions_const; wp.versions_value[0] = nb.versions_value[0]; wp.versions_value[1] = nb.versions_value[1];
+    wp.roles = dev + L.narrow.roles; wp.role_cols = nb.role_cols;
+    for (uint32_t v = 0; v < n_slots; v++) {
+        wp.slot_src[v] = dev + L.narrow.slot[v]; wp.slot_class[v] = nb.slot_class[v];
+        wp.slot_base[v] = nb.slot_base ? nb.slot_base[v] : 0u; wp.slot_base2[v] = nb.slot_base2 ? nb.slot_base2[v] : 0u;
+    }
+    wp.hdr0 = reinterpret_cast<cb_hdr0 *>(dev + L.col[CGPU_COL_HDR0]); wp.hdr1 = reinterpret_cast<cb_hdr1 *>(dev + L.col[CGPU_COL_HDR1]);
+    wp.roles_out = reinterpret_cast<uint32_t *>(dev + L.col[CGPU_COL_ROLES]); wp.slots_out = reinterpret_cast<uint64_t *>(dev + L.col[CGPU_COL_SLOTS]);
+    wp.stride = N; wp.n_slots = n_slots;
+    return wp;
+}
+
+// Requests [first, first + count): their narrow columns go H2D into the staging; once they have landed, widened on `stream`
+int upload_narrow_chunk(const cgpu_narrow &nb, WidenParams &wp, uint64_t first, uint64_t count, cudaStream_t h2d, cudaEvent_t landed, cudaStream_t stream,
+                        std::atomic<uint64_t> &launches) {
+    auto copy = [&](const void *staged, const void *src, size_t bytes) { return cudaMemcpyAsync(const_cast<void *>(staged), src, bytes, cudaMemcpyHostToDevice, h2d); };
+    if (nb.principal_id16) CUDA_TRY(copy(wp.pid16 + first, nb.principal_id16 + first, count * 2));
+    else CUDA_TRY(copy(wp.pid + first, nb.principal_id + first, count * 4));
+    if (wp.hdr_w) CUDA_TRY(copy(wp.hdr16 + first * wp.hdr_w, nb.hdr16 + first * wp.hdr_w, count * 2 * wp.hdr_w));
+    if (!nb.versions_const) CUDA_TRY(copy(wp.versions + first * 2, nb.versions + first * 2, count * 2));
+    for (uint32_t i = 0; i < nb.role_cols; i++) CUDA_TRY(copy(wp.roles + i * wp.stride + first, nb.roles + i * wp.stride + first, count));
+    for (uint32_t v = 0; v < wp.n_slots; v++) {
+        const uint32_t es = kNarrowElemBytes[wp.slot_class[v]];
+        CUDA_TRY(copy(static_cast<const uint8_t *>(wp.slot_src[v]) + first * es, static_cast<const uint8_t *>(nb.slot_cols[v]) + first * es, count * es));
+    }
+    CUDA_TRY(cudaEventRecord(landed, h2d));
+    CUDA_TRY(cudaStreamWaitEvent(stream, landed, 0));
+    wp.first = first; wp.count = count;
+    const uint64_t tiles = (count + kThreads - 1) / kThreads;
+    widen_kernel<<<(unsigned)(tiles < 1184 ? tiles : 1184), kThreads, 0, stream>>>(wp);
+    CUDA_TRY(cudaGetLastError());
+    launches.fetch_add(1, std::memory_order_relaxed);
+    return CGPU_OK;
+}
+
 // unique-condition kernels (cb_uc.h image; generic condition evaluator; deferrals go to the launch's list)
 template <bool kStaged>
 __global__ void __launch_bounds__(kThreads, CB_MIN_BLOCKS) check_uc(const __grid_constant__ TableDesc td, const __grid_constant__ cb::BatchView bv, uint8_t *bitmap,
@@ -346,24 +420,7 @@ __global__ void __launch_bounds__(kThreads) cluster_scatter(const __grid_constan
     }
 }
 
-// ------------------------------------------------------------------------------------------------ host side
-thread_local std::string g_err;
-
-int fail(int code, const char *fmt, ...) {
-    char buf[512];
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(buf, sizeof(buf), fmt, ap);
-    va_end(ap);
-    g_err = buf;
-    return code;
-}
-#define CUDA_TRY(expr)                                                                                   \
-    do {                                                                                                 \
-        cudaError_t e__ = (expr);                                                                        \
-        if (e__ != cudaSuccess) return fail(CGPU_ERR_CUDA, "%s failed: %s", #expr, cudaGetErrorString(e__)); \
-    } while (0)
-
+// ------------------------------------------------------------------------------------------- host side: check launches
 struct Slot {   // per in-flight cgpu_check call
     cudaStream_t stream = nullptr;                 // kernels
     cudaStream_t h2d = nullptr, d2h = nullptr;     // column chunks in, effect bytes out (PCIe is full duplex)
@@ -970,6 +1027,17 @@ cudaError_t launch_serialised(const void *fn, uint32_t grid, uint32_t block, uin
     return cudaLaunchKernelExC(&cfg, fn, args);
 }
 
+// A reference-order kernel (a thread per request, grid-stride) over `count` requests: -> its grid, or a CGPU_ERR_* code (< 0)
+template <class... Params, class... Args>
+int launch_reference(cgpu_ctx *ctx, void (*kernel)(Params...), uint64_t count, cudaStream_t stream, Args... args) {
+    const uint64_t tiles = (count + kThreads - 1) / kThreads, gmax = (uint64_t)ctx->sm_count * 4;
+    const uint32_t grid = (uint32_t)(tiles < gmax ? tiles : gmax);
+    kernel<<<grid, kThreads, 0, stream>>>(args...);
+    CUDA_TRY(cudaGetLastError());
+    ctx->launches.fetch_add(1, std::memory_order_relaxed);
+    return (int)grid;
+}
+
 // Issues the launches of `plan` (plan_launch for this table and batch) on `stream`.  md: the metadata form of the plan's
 // unique-condition kernel (cbuc::build_meta's table must exist), its deferrals drained by check_meta_kernel.
 int launch_check(cgpu_ctx *ctx, const cgpu_table *t, const LaunchPlan &plan_in, const cb::BatchView &bv, uint8_t *d_bitmap, uint8_t *d_effects,
@@ -1052,10 +1120,8 @@ int launch_check(cgpu_ctx *ctx, const cgpu_table *t, const LaunchPlan &plan_in, 
         cb::BatchView dv = bv;
         dv.perm = defer;
         dv.count_dev = bvv.defer_count;
-        const uint64_t gmax = (uint64_t)ctx->sm_count * 4;
-        check_meta_kernel<<<(unsigned)(tiles < gmax ? tiles : gmax), kThreads, 0, stream>>>(t->desc, dv, d_effects, d_am, d_rm, d_status);
-        CUDA_TRY(cudaGetLastError());
-        ctx->launches.fetch_add(1, std::memory_order_relaxed);
+        const int rc = launch_reference(ctx, check_meta_kernel, bv.count, stream, t->desc, dv, d_effects, d_am, d_rm, d_status);
+        if (rc < 0) return rc;
     } else if (plan.lean) {
         // drain the deferral list with the general body (usually empty: the kernel then exits at once); it also does the
         // fused-gather signalling (BatchView::sig_*)
@@ -1722,35 +1788,91 @@ struct MetaOut {
 static constexpr size_t kOutputSlabBytes = 256ull << 20;
 static constexpr uint32_t kMaxOutputStride = (uint32_t)(kOutputSlabBytes / 2 / 256);   // a chunk keeps at least 256 requests
 
-// requests [lo, hi) of `batch` on ctx's device: pipelined H2D / kernels / D2H (see below); effects_out covers the whole batch.
-// meta: also the metadata plane, from check_meta_kernel in place of the check kernels (nullptr: effects only)
-static inline uint32_t narrow_elem_bytes(uint32_t cl) {
-    return cl == CGPU_SLOT_U64 ? 8u : (cl == CGPU_SLOT_U8 || cl == CGPU_SLOT_U8_NUM) ? 1u : cl == CGPU_SLOT_U16_ID ? 2u : 4u;
+static inline size_t round256(size_t n) { return (n + 255) & ~(size_t)255; }
+
+// The batch a narrow batch stands for on the device: its per-request columns and heap at their canonical (widened) sizes,
+// in cols / bytes; a null column gets a placeholder
+static cgpu_batch canonical_batch(const cgpu_batch &b, const cgpu_narrow &nb, uint32_t n_slots, const void **cols, size_t *bytes) {
+    const uint64_t N = b.n_requests;
+    for (int i = 0; i < CGPU_N_COLUMNS; i++) { bytes[i] = b.column_bytes[i]; cols[i] = b.columns[i] ? b.columns[i] : static_cast<const void *>(""); }
+    bytes[CGPU_COL_HDR0] = N * sizeof(cb_hdr0); bytes[CGPU_COL_HDR1] = N * sizeof(cb_hdr1);
+    bytes[CGPU_COL_ROLES] = (size_t)nb.role_cols * N * 4;
+    bytes[CGPU_COL_SLOTS] = (size_t)(n_slots ? n_slots : 1) * N * 8;
+    bytes[CGPU_COL_HEAP] *= nb.heap_bits == 16 ? 4 : nb.heap_u32 ? 2 : 1;   // 16- / 32-bit heap words widen to 64 bits
+    cgpu_batch c = b;
+    c.columns = cols; c.column_bytes = bytes;
+    return c;
 }
+
+static SlotLayout slot_layout(const cgpu_batch &b, const cgpu_narrow *nb, size_t narrow_heap_bytes, uint32_t n_slots, const MetaOut *meta) {
+    SlotLayout L{};
+    auto take = [&](size_t bytes) { const size_t at = L.total; L.total += round256(bytes); return at; };
+    const uint64_t N = b.n_requests;
+    const uint32_t km = b.max_actions ? b.max_actions : 1;
+    for (int i = 0; i < CGPU_N_COLUMNS; i++) L.col[i] = take(b.column_bytes[i]);
+    L.effects = take(N * km);
+    if (nb) {
+        L.narrow.pid = take(N * (nb->principal_id16 ? 2 : 4));
+        L.narrow.hdr16 = take(N * 2 * narrow_hdr_w(*nb));
+        L.narrow.versions = take(nb->versions_const ? 0 : N * 2);
+        L.narrow.roles = take((size_t)nb->role_cols * N);
+        for (uint32_t v = 0; v < n_slots; v++) L.narrow.slot[v] = take(N * kNarrowElemBytes[nb->slot_class[v]]);
+        if (nb->heap_u32 || nb->heap_bits) L.narrow.heap = take(narrow_heap_bytes);
+    }
+    if (meta) { L.action_meta = take(N * km * 4); L.request_meta = take(N * sizeof(cb_request_meta)); }
+    if (meta && meta->outputs) {
+        L.out_chunk = (kOutputSlabBytes / 2 / meta->stride) & ~(uint64_t)255;
+        L.needed = take(4);
+        L.out = take(2 * L.out_chunk * meta->stride);
+    }
+    return L;
+}
+
+// Requests [first, first + count) of a wide batch: their columns go H2D from host view to device view; the kernels wait for them
+static int upload_chunk(const cb::BatchView &hv, const cb::BatchView &dv, uint32_t n_slots, uint64_t first, uint64_t count, const Slot &slot, cudaEvent_t landed) {
+    auto copy = [&](const void *dst, const void *src, size_t bytes) { return cudaMemcpyAsync(const_cast<void *>(dst), src, bytes, cudaMemcpyHostToDevice, slot.h2d); };
+    CUDA_TRY(copy(dv.hdr0 + first, hv.hdr0 + first, count * sizeof(cb_hdr0)));
+    CUDA_TRY(copy(dv.hdr1 + first, hv.hdr1 + first, count * sizeof(cb_hdr1)));
+    for (uint32_t i = 0; i < dv.role_cols; i++) CUDA_TRY(copy(dv.roles + i * dv.stride + first, hv.roles + i * hv.stride + first, count * 4));
+    for (uint32_t v = 0; v < n_slots; v++) CUDA_TRY(copy(dv.slots + v * dv.stride + first, hv.slots + v * hv.stride + first, count * 8));
+    CUDA_TRY(cudaEventRecord(landed, slot.h2d));
+    CUDA_TRY(cudaStreamWaitEvent(slot.stream, landed, 0));
+    return CGPU_OK;
+}
+
+// Evaluates chunk cv on `stream`, effect bytes written directly.  Rule outputs (into `slab`): the reference-order body, whose
+// row order they follow.  Metadata: the effect plan's unique-condition kernel in metadata form where the table has the side
+// table it reads, else the reference-order body.  Effects alone: the effect launch.
+static int launch_chunk(cgpu_ctx *ctx, const cgpu_table *t, const cb::BatchView &cv, const MetaOut *meta, uint8_t *dev, const SlotLayout &L, uint8_t *slab,
+                        uint32_t *d_status, cudaStream_t stream) {
+    uint8_t *d_effects = dev + L.effects;
+    if (!meta) return launch_check(ctx, t, plan_launch(*ctx, *t, cv), cv, nullptr, d_effects, d_status, stream);
+    uint32_t *d_am = reinterpret_cast<uint32_t *>(dev + L.action_meta);
+    cb_request_meta *d_rm = reinterpret_cast<cb_request_meta *>(dev + L.request_meta);
+    const LaunchPlan plan = meta->outputs ? LaunchPlan() : plan_launch(*ctx, *t, cv);
+    const MetaDev md{d_am, d_rm};
+    if (plan.uc && t->d_uc_meta) return launch_check(ctx, t, plan, cv, nullptr, d_effects, d_status, stream, &md);
+    const int grid = meta->outputs ? launch_reference(ctx, check_outputs_kernel, cv.count, stream, t->desc, cv, d_effects, d_am, d_rm, d_status, slab,
+                                                      meta->stride, reinterpret_cast<uint32_t *>(dev + L.needed))
+                                   : launch_reference(ctx, check_meta_kernel, cv.count, stream, t->desc, cv, d_effects, d_am, d_rm, d_status);
+    if (grid < 0) return grid;
+    ctx->last_plan = LaunchPlan();   // (general body, no unique-condition kernel)
+    ctx->last_grid = (uint32_t)grid;
+    return CGPU_OK;
+}
+
+// requests [lo, hi) of `batch` on ctx's device: pipelined H2D / kernels / D2H (see below); effects_out covers the whole batch.
+// meta: also the metadata planes (and rule outputs), nullptr: effects only.  nb: the batch is in the narrow form (valid).
 static int check_range(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch_in, uint64_t lo, uint64_t hi, uint8_t *effects_out, const cgpu_narrow *nb,
                        const MetaOut *meta) {
-    // narrow form: the canonical sizes of the per-request columns (and of a 32-bit heap) are implied, not passed
-    cgpu_batch batch_c = *batch_in;
-    size_t cbytes[CGPU_N_COLUMNS];
+    const uint32_t n_slots = t->desc.lay.n_slots;
     const void *ccols[CGPU_N_COLUMNS];
-    uint32_t n_role_cols_narrow = 0;
-    if (nb) {
-        for (int i = 0; i < CGPU_N_COLUMNS; i++) { cbytes[i] = batch_in->column_bytes[i]; ccols[i] = batch_in->columns[i] ? batch_in->columns[i] : static_cast<const void *>(""); }
-        n_role_cols_narrow = nb->role_cols;
-        cbytes[CGPU_COL_HDR0] = batch_in->n_requests * 16; cbytes[CGPU_COL_HDR1] = batch_in->n_requests * 8;
-        cbytes[CGPU_COL_ROLES] = (size_t)nb->role_cols * batch_in->n_requests * 4;
-        cbytes[CGPU_COL_SLOTS] = (size_t)(t->desc.lay.n_slots ? t->desc.lay.n_slots : 1) * batch_in->n_requests * 8;
-        if (nb->heap_bits == 16) cbytes[CGPU_COL_HEAP] = batch_in->column_bytes[CGPU_COL_HEAP] * 4;
-        else if (nb->heap_bits != 0) return fail(CGPU_ERR_INVALID, "cgpu_check_narrow: heap_bits %u (0 or 16)", nb->heap_bits);
-        else if (nb->heap_u32) cbytes[CGPU_COL_HEAP] = batch_in->column_bytes[CGPU_COL_HEAP] * 2;
-        batch_c.columns = ccols; batch_c.column_bytes = cbytes;
-    }
-    const cgpu_batch *batch = &batch_c;
-    (void)n_role_cols_narrow;
-    const uint64_t N = batch->n_requests;
-    const uint32_t km = batch->max_actions ? batch->max_actions : 1;
+    size_t cbytes[CGPU_N_COLUMNS];
+    const cgpu_batch batch = nb ? canonical_batch(*batch_in, *nb, n_slots, ccols, cbytes) : *batch_in;
+    const uint64_t N = batch.n_requests;
+    const uint32_t km = batch.max_actions ? batch.max_actions : 1;
     cb::BatchView hv;
-    int rc = invalid(cbhost::make_batch_view(t->desc.lay, batch, 0, N, &hv));   // validates sizes (pointers here are host pointers)
+    int rc = invalid(cbhost::make_batch_view(t->desc.lay, &batch, 0, N, &hv));   // validates sizes (pointers here are host pointers)
     if (rc != CGPU_OK) return rc;
     CUDA_TRY(cudaSetDevice(ctx->device));
 
@@ -1775,63 +1897,21 @@ static int check_range(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *bat
     // a failed call must not leave work queued on the slot's streams when the slot goes back to the pool
     struct Quiesce { Slot *s; bool armed = true; ~Quiesce() { if (armed) { cudaStreamSynchronize(s->h2d); cudaStreamSynchronize(s->stream); cudaStreamSynchronize(s->d2h); } } } quiesce{slot};
 
-    // device layout: every column 256-byte aligned, then the effect bytes
-    size_t offs[CGPU_N_COLUMNS + 1];
-    size_t total = 0;
-    for (int i = 0; i < CGPU_N_COLUMNS; i++) { offs[i] = total; total += (batch->column_bytes[i] + 255) & ~(size_t)255; }
-    const size_t eff_bytes = (size_t)N * km;
-    offs[CGPU_N_COLUMNS] = total;
-    total += (eff_bytes + 255) & ~(size_t)255;
-    // narrow form: staging for the narrow columns (and the 32-bit heap) behind the canonical region
-    size_t n_pid = 0, n_h16 = 0, n_ver = 0, n_roles = 0, n_heap32 = 0, n_slot[kMaxNarrowSlots] = {0};
-    const uint32_t n_slots_t = t->desc.lay.n_slots;
-    const uint32_t hdr_w = nb ? 4u - (uint32_t)__builtin_popcount(nb->hdr_const_mask & 15u) : 4u;   // header fields that travel
-    if (nb) {
-        if (n_slots_t > kMaxNarrowSlots) return fail(CGPU_ERR_INVALID, "cgpu_check_narrow: more than %u attribute slots", kMaxNarrowSlots);
-        auto take = [&](size_t bytes) { const size_t at = total; total += (bytes + 255) & ~(size_t)255; return at; };
-        if ((nb->hdr_const_mask & ~15u) || (hdr_w && !nb->hdr16) || (!nb->versions_const && !nb->versions) || (!nb->principal_id16 && !nb->principal_id))
-            return fail(CGPU_ERR_INVALID, "cgpu_check_narrow: missing narrow column");
-        n_pid = take(N * (nb->principal_id16 ? 2 : 4)); n_h16 = take(N * 2 * hdr_w); n_ver = take(nb->versions_const ? 0 : N * 2); n_roles = take((size_t)nb->role_cols * N);
-        for (uint32_t v = 0; v < n_slots_t; v++) {
-            const uint32_t cl = nb->slot_class[v];
-            if (cl > CGPU_SLOT_U8_NUM) return fail(CGPU_ERR_INVALID, "cgpu_check_narrow: slot class %u", cl);
-            if (cl == CGPU_SLOT_U16_ID && !nb->slot_base) return fail(CGPU_ERR_INVALID, "cgpu_check_narrow: CGPU_SLOT_U16_ID needs slot_base");
-            n_slot[v] = take(N * narrow_elem_bytes(cl));
-        }
-        if (nb->heap_u32 || nb->heap_bits) n_heap32 = take(batch_in->column_bytes[CGPU_COL_HEAP]);
-    }
-    // metadata plane: the action words and the request records
-    size_t off_am = 0, off_rm = 0;
-    if (meta) {
-        off_am = total; total += ((size_t)N * km * 4 + 255) & ~(size_t)255;
-        off_rm = total; total += ((size_t)N * sizeof(cb_request_meta) + 255) & ~(size_t)255;
-    }
-    const bool outs = meta && meta->outputs;
-    // output records: two slabs of `chunk` records (chunk below is cut to fit kOutputSlabBytes) and the needed-size word
-    uint64_t out_chunk = 0;
-    size_t off_out = 0, off_need = 0;
-    if (outs) {
-        out_chunk = (kOutputSlabBytes / 2 / meta->stride) & ~(uint64_t)255;
-        off_need = total; total += 256;
-        off_out = total; total += 2 * out_chunk * meta->stride;
-    }
-    if (slot->dev_cap < total) {
+    const SlotLayout L = slot_layout(batch, nb, batch_in->column_bytes[CGPU_COL_HEAP], n_slots, meta);
+    if (slot->dev_cap < L.total) {
         if (slot->dev) cudaFree(slot->dev);
         slot->dev = nullptr; slot->dev_cap = 0;
-        CUDA_TRY(cudaMalloc(&slot->dev, total));
-        slot->dev_cap = total;
+        CUDA_TRY(cudaMalloc(&slot->dev, L.total));
+        slot->dev_cap = L.total;
     }
-    uint8_t *dbase = static_cast<uint8_t *>(slot->dev);
+    uint8_t *dev = static_cast<uint8_t *>(slot->dev);
     const void *dcols[CGPU_N_COLUMNS];
-    for (int i = 0; i < CGPU_N_COLUMNS; i++) dcols[i] = dbase + offs[i];
-    cgpu_batch db = *batch;
+    for (int i = 0; i < CGPU_N_COLUMNS; i++) dcols[i] = dev + L.col[i];
+    cgpu_batch db = batch;
     db.columns = dcols;
     cb::BatchView bv;
     rc = invalid(cbhost::make_batch_view(t->desc.lay, &db, 0, N, &bv));
     if (rc != CGPU_OK) return rc;
-    uint8_t *d_effects = dbase + offs[CGPU_N_COLUMNS];
-    uint32_t *d_am = reinterpret_cast<uint32_t *>(dbase + off_am);
-    cb_request_meta *d_rm = reinterpret_cast<cb_request_meta *>(dbase + off_rm);
 
     // Pipeline: the batch-level tables and the heap go first, then the per-request columns travel in chunks of
     // `chunk` requests -- while chunk k is evaluated, chunk k+1 is on its way in and the effect bytes of chunk k-1 on
@@ -1841,139 +1921,66 @@ static int check_range(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *bat
     // Chunk size: every column of a chunk is one copy, so chunks must be large for the link to run near its rate -- measured
     // on C3's narrow form (52 B / request): 2^18 requests 38 GB/s, 2^19 42.5, 2^20 44.8, 2^21 46.3, 2^22 44.6
     // (tools/e2e_chunk_sweep.py) -- but a call should still be cut in two so that copy-in, kernels and copy-out overlap.
+    const bool outs = meta && meta->outputs;
     const char *ce = getenv("CERBOS_B200_CHECK_CHUNK");
     uint64_t chunk = ce ? strtoull(ce, nullptr, 10) : (1ull << 21);
     if (!ce && hi - lo < 2 * chunk) {
         chunk = (hi - lo + 1) / 2;
         if (chunk < (1ull << 18)) chunk = 1ull << 18;
-        chunk = (chunk + 255) & ~(uint64_t)255;
+        chunk = round256(chunk);
     }
     if (chunk < 4096) chunk = 4096;
     chunk &= ~(uint64_t)255;
-    if (outs && chunk > out_chunk) chunk = out_chunk;
+    if (outs && chunk > L.out_chunk) chunk = L.out_chunk;
     const uint64_t n_chunks = (hi - lo + chunk - 1) / chunk;
     const uint64_t n_ev = (outs ? 3 : 2) * n_chunks;   // per chunk: columns in, kernel done, (outputs) output slab drained
-    uint32_t *d_need = reinterpret_cast<uint32_t *>(dbase + off_need);
-    uint8_t *d_out = dbase + off_out;
-    if (outs) CUDA_TRY(cudaMemsetAsync(d_need, 0, 4, slot->stream));
+    if (outs) CUDA_TRY(cudaMemsetAsync(dev + L.needed, 0, 4, slot->stream));
     while (slot->ev.size() < n_ev) {
         cudaEvent_t e;
         CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
         slot->ev.push_back(e);
     }
-    const uint8_t *const *hc = reinterpret_cast<const uint8_t *const *>(batch->columns);
-    for (int i = CGPU_COL_HEAP; i < CGPU_N_COLUMNS; i++) {
-        if (nb && (nb->heap_u32 || nb->heap_bits) && i == CGPU_COL_HEAP) {
-            const size_t nb32 = batch_in->column_bytes[CGPU_COL_HEAP];
-            if (nb32) {
-                CUDA_TRY(cudaMemcpyAsync(dbase + n_heap32, hc[i], nb32, cudaMemcpyHostToDevice, slot->h2d));
-                const uint64_t words = nb32 / (nb->heap_bits == 16 ? 2 : 4);
-                const unsigned hgrid = (unsigned)((words + kThreads - 1) / kThreads < 1184 ? (words + kThreads - 1) / kThreads : 1184);
-                if (nb->heap_bits == 16)
-                    widen_heap16_kernel<<<hgrid, kThreads, 0, slot->h2d>>>(reinterpret_cast<const uint16_t *>(dbase + n_heap32), reinterpret_cast<uint64_t *>(dbase + offs[i]), words, nb->heap_base, nb->heap_base2);
-                else
-                widen_heap_kernel<<<hgrid, kThreads, 0, slot->h2d>>>(
-                    reinterpret_cast<const uint32_t *>(dbase + n_heap32), reinterpret_cast<uint64_t *>(dbase + offs[i]), words);
-                CUDA_TRY(cudaGetLastError());
-                ctx->launches.fetch_add(1, std::memory_order_relaxed);
-            }
-            continue;
-        }
-        if (batch->column_bytes[i]) CUDA_TRY(cudaMemcpyAsync(dbase + offs[i], hc[i], batch->column_bytes[i], cudaMemcpyHostToDevice, slot->h2d));
+    // the batch-level tables and the heap, once per call; a 16- or 32-bit heap is widened into the canonical one on the copy stream
+    const bool narrow_heap = nb && (nb->heap_u32 || nb->heap_bits);
+    if (const size_t hb = narrow_heap ? batch_in->column_bytes[CGPU_COL_HEAP] : 0) {
+        CUDA_TRY(cudaMemcpyAsync(dev + L.narrow.heap, batch.columns[CGPU_COL_HEAP], hb, cudaMemcpyHostToDevice, slot->h2d));
+        const uint64_t words = hb / (nb->heap_bits == 16 ? 2 : 4), tiles = (words + kThreads - 1) / kThreads;
+        const unsigned hgrid = (unsigned)(tiles < 1184 ? tiles : 1184);
+        uint64_t *heap = reinterpret_cast<uint64_t *>(dev + L.col[CGPU_COL_HEAP]);
+        if (nb->heap_bits == 16) widen_heap16_kernel<<<hgrid, kThreads, 0, slot->h2d>>>(reinterpret_cast<const uint16_t *>(dev + L.narrow.heap), heap, words, nb->heap_base, nb->heap_base2);
+        else widen_heap_kernel<<<hgrid, kThreads, 0, slot->h2d>>>(reinterpret_cast<const uint32_t *>(dev + L.narrow.heap), heap, words);
+        CUDA_TRY(cudaGetLastError());
+        ctx->launches.fetch_add(1, std::memory_order_relaxed);
     }
+    for (int i = narrow_heap ? CGPU_COL_HEAP + 1 : CGPU_COL_HEAP; i < CGPU_N_COLUMNS; i++)
+        if (batch.column_bytes[i]) CUDA_TRY(cudaMemcpyAsync(dev + L.col[i], batch.columns[i], batch.column_bytes[i], cudaMemcpyHostToDevice, slot->h2d));
+    WidenParams wp{};
+    if (nb) wp = widen_params(*nb, N, n_slots, dev, L);
     for (uint64_t k = 0; k < n_chunks; k++) {
         const uint64_t c0 = lo + k * chunk, cnt = hi - c0 < chunk ? hi - c0 : chunk;
-        if (nb) {
-            if (nb->principal_id16) CUDA_TRY(cudaMemcpyAsync(dbase + n_pid + c0 * 2, nb->principal_id16 + c0, cnt * 2, cudaMemcpyHostToDevice, slot->h2d));
-            else CUDA_TRY(cudaMemcpyAsync(dbase + n_pid + c0 * 4, nb->principal_id + c0, cnt * 4, cudaMemcpyHostToDevice, slot->h2d));
-            if (hdr_w) CUDA_TRY(cudaMemcpyAsync(dbase + n_h16 + c0 * 2 * hdr_w, nb->hdr16 + c0 * hdr_w, cnt * 2 * hdr_w, cudaMemcpyHostToDevice, slot->h2d));
-            if (!nb->versions_const) CUDA_TRY(cudaMemcpyAsync(dbase + n_ver + c0 * 2, nb->versions + c0 * 2, cnt * 2, cudaMemcpyHostToDevice, slot->h2d));
-            for (uint32_t i = 0; i < nb->role_cols; i++)
-                CUDA_TRY(cudaMemcpyAsync(dbase + n_roles + (uint64_t)i * N + c0, nb->roles + (uint64_t)i * N + c0, cnt, cudaMemcpyHostToDevice, slot->h2d));
-            WidenParams wp{};
-            for (uint32_t v = 0; v < n_slots_t; v++) {
-                const uint32_t cl = nb->slot_class[v], es = narrow_elem_bytes(cl);
-                CUDA_TRY(cudaMemcpyAsync(dbase + n_slot[v] + c0 * es, static_cast<const uint8_t *>(nb->slot_cols[v]) + c0 * es, cnt * es, cudaMemcpyHostToDevice, slot->h2d));
-                wp.slot_src[v] = dbase + n_slot[v];
-                wp.slot_class[v] = (uint8_t)cl;
-                wp.slot_base[v] = nb->slot_base ? nb->slot_base[v] : 0u;
-                wp.slot_base2[v] = nb->slot_base2 ? nb->slot_base2[v] : 0u;
-            }
-            wp.pid16 = nb->principal_id16 ? reinterpret_cast<const uint16_t *>(dbase + n_pid) : nullptr; wp.pid_base = nb->principal_base;
-            wp.hdr_const_mask = nb->hdr_const_mask & 15u; wp.hdr_w = hdr_w;
-            for (int f = 0; f < 4; f++) wp.hdr_const[f] = nb->hdr_const[f];
-            wp.versions_const = nb->versions_const; wp.versions_value[0] = nb->versions_value[0]; wp.versions_value[1] = nb->versions_value[1];
-            wp.pid = reinterpret_cast<const uint32_t *>(dbase + n_pid); wp.hdr16 = reinterpret_cast<const uint16_t *>(dbase + n_h16);
-            wp.versions = dbase + n_ver; wp.roles = dbase + n_roles;
-            wp.hdr0 = reinterpret_cast<cb_hdr0 *>(dbase + offs[CGPU_COL_HDR0]); wp.hdr1 = reinterpret_cast<cb_hdr1 *>(dbase + offs[CGPU_COL_HDR1]);
-            wp.roles_out = reinterpret_cast<uint32_t *>(dbase + offs[CGPU_COL_ROLES]); wp.slots_out = reinterpret_cast<uint64_t *>(dbase + offs[CGPU_COL_SLOTS]);
-            wp.first = c0; wp.count = cnt; wp.stride = N; wp.role_cols = nb->role_cols; wp.n_slots = n_slots_t;
-            CUDA_TRY(cudaEventRecord(slot->ev[2 * k], slot->h2d));
-            CUDA_TRY(cudaStreamWaitEvent(slot->stream, slot->ev[2 * k], 0));
-            const uint64_t wt = (cnt + kThreads - 1) / kThreads;
-            widen_kernel<<<(unsigned)(wt < 1184 ? wt : 1184), kThreads, 0, slot->stream>>>(wp);
-            CUDA_TRY(cudaGetLastError());
-            ctx->launches.fetch_add(1, std::memory_order_relaxed);
-        } else {
-        CUDA_TRY(cudaMemcpyAsync(dbase + offs[CGPU_COL_HDR0] + c0 * 16, hc[CGPU_COL_HDR0] + c0 * 16, cnt * 16, cudaMemcpyHostToDevice, slot->h2d));
-        CUDA_TRY(cudaMemcpyAsync(dbase + offs[CGPU_COL_HDR1] + c0 * 8, hc[CGPU_COL_HDR1] + c0 * 8, cnt * 8, cudaMemcpyHostToDevice, slot->h2d));
-        for (uint32_t i = 0; i < bv.role_cols; i++)
-            CUDA_TRY(cudaMemcpyAsync(dbase + offs[CGPU_COL_ROLES] + ((uint64_t)i * N + c0) * 4, hc[CGPU_COL_ROLES] + ((uint64_t)i * N + c0) * 4, cnt * 4, cudaMemcpyHostToDevice, slot->h2d));
-        for (uint32_t v = 0; v < t->desc.lay.n_slots; v++)
-            CUDA_TRY(cudaMemcpyAsync(dbase + offs[CGPU_COL_SLOTS] + ((uint64_t)v * N + c0) * 8, hc[CGPU_COL_SLOTS] + ((uint64_t)v * N + c0) * 8, cnt * 8, cudaMemcpyHostToDevice, slot->h2d));
-        CUDA_TRY(cudaEventRecord(slot->ev[2 * k], slot->h2d));
-        CUDA_TRY(cudaStreamWaitEvent(slot->stream, slot->ev[2 * k], 0));
-        }
+        rc = nb ? upload_narrow_chunk(*nb, wp, c0, cnt, slot->h2d, slot->ev[2 * k], slot->stream, ctx->launches)
+                : upload_chunk(hv, bv, n_slots, c0, cnt, *slot, slot->ev[2 * k]);
+        if (rc != CGPU_OK) return rc;
         cb::BatchView cv = bv;
         cv.first = c0; cv.count = cnt;
-        // the kernel writes effect bytes directly (1 ALLOW / 2 DENY / 0 padding): no host post-pass
-        if (outs) {
-            // always the reference-order body: outputs come from the rows it visits, in its order
-            uint8_t *slab = d_out + (k & 1) * out_chunk * meta->stride;
-            if (k >= 2) CUDA_TRY(cudaStreamWaitEvent(slot->stream, slot->ev[2 * n_chunks + k - 2], 0));   // that slab's last copy-out
-            const uint64_t tiles = (cnt + kThreads - 1) / kThreads;
-            const uint32_t grid = (uint32_t)(tiles < (uint64_t)ctx->sm_count * 4 ? tiles : (uint64_t)ctx->sm_count * 4);
-            check_outputs_kernel<<<grid, kThreads, 0, slot->stream>>>(t->desc, cv, d_effects, d_am, d_rm, slot->d_status, slab, meta->stride, d_need);
-            CUDA_TRY(cudaGetLastError());
-            ctx->launches.fetch_add(1, std::memory_order_relaxed);
-            ctx->last_plan = LaunchPlan();
-            ctx->last_grid = grid;
-        } else if (meta) {
-            // the unique-condition kernel the effect launch would run, in its metadata form, where the table has the side
-            // table that form reads; else the reference-order body for every request
-            const LaunchPlan plan = plan_launch(*ctx, *t, cv);
-            if (plan.uc && t->d_uc_meta) {
-                const MetaDev md{d_am, d_rm};
-                rc = launch_check(ctx, t, plan, cv, nullptr, d_effects, slot->d_status, slot->stream, &md);
-                if (rc != CGPU_OK) return rc;
-            } else {
-                const uint64_t tiles = (cnt + kThreads - 1) / kThreads;
-                const uint32_t grid = (uint32_t)(tiles < (uint64_t)ctx->sm_count * 4 ? tiles : (uint64_t)ctx->sm_count * 4);
-                check_meta_kernel<<<grid, kThreads, 0, slot->stream>>>(t->desc, cv, d_effects, d_am, d_rm, slot->d_status);
-                CUDA_TRY(cudaGetLastError());
-                ctx->launches.fetch_add(1, std::memory_order_relaxed);
-                ctx->last_plan = LaunchPlan();   // (general body, no unique-condition kernel)
-                ctx->last_grid = grid;
-            }
-        } else {
-            rc = launch_check(ctx, t, plan_launch(*ctx, *t, cv), cv, nullptr, d_effects, slot->d_status, slot->stream);
-            if (rc != CGPU_OK) return rc;
-        }
+        uint8_t *slab = outs ? dev + L.out + (k & 1) * L.out_chunk * meta->stride : nullptr;
+        if (outs && k >= 2) CUDA_TRY(cudaStreamWaitEvent(slot->stream, slot->ev[2 * n_chunks + k - 2], 0));   // that slab's last copy-out
+        rc = launch_chunk(ctx, t, cv, meta, dev, L, slab, slot->d_status, slot->stream);
+        if (rc != CGPU_OK) return rc;
         CUDA_TRY(cudaEventRecord(slot->ev[2 * k + 1], slot->stream));
         CUDA_TRY(cudaStreamWaitEvent(slot->d2h, slot->ev[2 * k + 1], 0));
-        CUDA_TRY(cudaMemcpyAsync(effects_out + c0 * km, d_effects + c0 * km, cnt * km, cudaMemcpyDeviceToHost, slot->d2h));
+        CUDA_TRY(cudaMemcpyAsync(effects_out + c0 * km, dev + L.effects + c0 * km, cnt * km, cudaMemcpyDeviceToHost, slot->d2h));
         if (meta) {
-            CUDA_TRY(cudaMemcpyAsync(meta->action_meta + c0 * km, d_am + c0 * km, cnt * km * 4, cudaMemcpyDeviceToHost, slot->d2h));
-            CUDA_TRY(cudaMemcpyAsync(meta->request_meta + c0, d_rm + c0, cnt * sizeof(cb_request_meta), cudaMemcpyDeviceToHost, slot->d2h));
+            CUDA_TRY(cudaMemcpyAsync(meta->action_meta + c0 * km, dev + L.action_meta + c0 * km * 4, cnt * km * 4, cudaMemcpyDeviceToHost, slot->d2h));
+            CUDA_TRY(cudaMemcpyAsync(meta->request_meta + c0, dev + L.request_meta + c0 * sizeof(cb_request_meta), cnt * sizeof(cb_request_meta), cudaMemcpyDeviceToHost, slot->d2h));
         }
         if (outs) {
-            const uint8_t *slab = d_out + (k & 1) * out_chunk * meta->stride;
             CUDA_TRY(cudaMemcpyAsync(meta->outputs + c0 * meta->stride, slab, cnt * meta->stride, cudaMemcpyDeviceToHost, slot->d2h));
             CUDA_TRY(cudaEventRecord(slot->ev[2 * n_chunks + k], slot->d2h));
         }
     }
     uint32_t h_need = 0;
-    if (outs) CUDA_TRY(cudaMemcpyAsync(&h_need, d_need, 4, cudaMemcpyDeviceToHost, slot->d2h));
+    if (outs) CUDA_TRY(cudaMemcpyAsync(&h_need, dev + L.needed, 4, cudaMemcpyDeviceToHost, slot->d2h));
     CUDA_TRY(cudaMemcpyAsync(slot->h_status, slot->d_status, 4, cudaMemcpyDeviceToHost, slot->d2h));   // behind the last chunk's results
     CUDA_TRY(cudaStreamSynchronize(slot->d2h));
     quiesce.armed = false;   // d2h waited for every kernel, every kernel for its columns: all three streams are idle
@@ -2022,12 +2029,21 @@ static int check_sharded(cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *b
     return CGPU_OK;
 }
 
-// the argument checks of the narrow entry points
-static int narrow_args(const char *fn, cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch, const cgpu_narrow *narrow, const uint8_t *effects_out) {
-    if (!ctx || !t || !batch || !narrow || !effects_out) return fail(CGPU_ERR_INVALID, "%s: null argument", fn);
+// the argument checks of the narrow entry points, the whole descriptor included, before any device work and at any batch size
+static int narrow_args(const char *fn, cgpu_ctx *ctx, const cgpu_table *t, const cgpu_batch *batch, const cgpu_narrow *nb, const uint8_t *effects_out) {
+    if (!ctx || !t || !batch || !nb || !effects_out) return fail(CGPU_ERR_INVALID, "%s: null argument", fn);
     if (t->ctx != ctx) return fail(CGPU_ERR_INVALID, "table belongs to another context");
-    if (!narrow->roles || !narrow->slot_class || !narrow->slot_cols || narrow->role_cols == 0)
+    if (!nb->roles || !nb->slot_class || !nb->slot_cols || nb->role_cols == 0 || (nb->hdr_const_mask & ~15u) || (narrow_hdr_w(*nb) && !nb->hdr16) ||
+        (!nb->versions_const && !nb->versions) || (!nb->principal_id16 && !nb->principal_id))
         return fail(CGPU_ERR_INVALID, "%s: missing narrow column", fn);
+    if (nb->heap_bits != 0 && nb->heap_bits != 16) return fail(CGPU_ERR_INVALID, "%s: heap_bits %u (0 or 16)", fn, nb->heap_bits);
+    const uint32_t n_slots = t->desc.lay.n_slots;
+    if (n_slots > kMaxNarrowSlots) return fail(CGPU_ERR_INVALID, "%s: more than %u attribute slots", fn, kMaxNarrowSlots);
+    for (uint32_t v = 0; v < n_slots; v++) {
+        const uint32_t cl = nb->slot_class[v];
+        if (cl > CGPU_SLOT_U8_NUM) return fail(CGPU_ERR_INVALID, "%s: slot class %u", fn, cl);
+        if (cl == CGPU_SLOT_U16_ID && !nb->slot_base) return fail(CGPU_ERR_INVALID, "%s: CGPU_SLOT_U16_ID needs slot_base", fn);
+    }
     return CGPU_OK;
 }
 

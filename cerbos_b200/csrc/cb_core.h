@@ -44,8 +44,10 @@ struct TableLayout {
     uint32_t nV, nRP, nS, nP, nR, nAP, nT, n_slots, n_rows;
     uint32_t has_role_policies, has_parent_roles, has_principal_policies;
     uint32_t image_bytes;
-    // "unique condition" image (cb_uc.h): offsets of the three derived sections, number of distinct conditions (0 = none)
+    // "unique condition" image (cb_uc.h): offsets of the three derived sections, number of condition records, one bit of the
+    // condition word each (0 = none): the distinct conditions, or the base conditions of a complement-coded image
     uint32_t uc_conds_off, uc_rows_off, uc_chain_off, n_uconds;
+    uint32_t uc_complement;                 // complement-coded: rows need each of their base conditions true or false
     uint32_t uc_n_rows;                     // merged records per action set: slots (segment form), else image rows
     uint32_t uc_slots_off;                  // segment form: the image row of every slot (CB_NONE32: unused), else 0
     uint32_t uc_deny_rows, uc_allow_rows;   // slots of every block's DENY / ALLOW segment (0 / 0: row ranges)
@@ -89,7 +91,7 @@ struct TableView {
     CB_HD const uint32_t *dr_name_str() const { return sec<uint32_t>(CB_SEC_DR_NAME_STR); }
     CB_HD const uint32_t *row_out() const { return sec<uint32_t>(CB_SEC_ROW_OUT); }            // tables with rule outputs only
     CB_HD const cb_out_entry *out_entries() const { return sec<cb_out_entry>(CB_SEC_OUT_ENTRIES); }
-    CB_HD const cb_cond *uconds() const { return reinterpret_cast<const cb_cond *>(base + L->uc_conds_off); }     // [n_uconds + 1]; entry 0: {rows of the longest scope, 0, 0, 0} (cb_uc.h)
+    CB_HD const cb_cond *uconds() const { return reinterpret_cast<const cb_cond *>(base + L->uc_conds_off); }     // [n_uconds + 1]; entry 0: {rows of the longest scope, DENY / ALLOW slots, ..} (cb_uc.h)
     CB_HD const U4 *urows() const { return reinterpret_cast<const U4 *>(base + L->uc_rows_off); }                 // [n_rows] 16-byte rows, DENY first per block
     CB_HD const uint32_t *uc_slots() const { return reinterpret_cast<const uint32_t *>(base + L->uc_slots_off); }  // [uc_n_rows] segment form: image row per slot
     CB_HD const U4 *uc_chain() const { return reinterpret_cast<const U4 *>(base + L->uc_chain_off); }             // like RES_BLOCK_MAP: one scope-walk step each
@@ -4892,9 +4894,10 @@ struct CachedCols {
 // How the unique-condition body gets a request's condition word: this generic evaluator interprets the table's DNF
 // terms; a run-time
 // specialised build (cb_specialize.h: generate_uc) substitutes straight-line code over register-resident slots.
-// The condition word: bit u = distinct condition u holds, bit 0 = "no condition".  Form 0: at most 32 bits, rows carry a
-// 32-bit need mask; form 1: 64 bits, 64-bit need masks; form 2 (64..127 distinct conditions, run-time specialised
-// kernels only): rows carry the two condition NUMBERS they need instead of a mask.
+// The condition word: bit u = condition u holds, bit 0 = "no condition"; its conditions are the image's records (cb_uc.h):
+// the base conditions of a complement-coded image, else the distinct conditions.  Form 0: at most 32 bits, rows carry a
+// need-true mask and a need-false mask (0 unless complement-coded); form 1: 64 bits, 64-bit need masks; form 2 (64..127
+// distinct conditions, run-time specialised kernels only): rows carry the two condition NUMBERS they need instead of a mask.
 struct CondWord { uint64_t lo, hi; };
 enum { CB_UC_FORM_MASK32 = 0, CB_UC_FORM_MASK64 = 1, CB_UC_FORM_INDEX = 2 };
 // Rows of one scope up to which a table-specialised walk is fully unrolled: the DENY + ALLOW slots of the image's segment
@@ -4902,7 +4905,9 @@ enum { CB_UC_FORM_MASK32 = 0, CB_UC_FORM_MASK64 = 1, CB_UC_FORM_INDEX = 2 };
 constexpr uint32_t kUcUnrollRows = 16;
 constexpr uint32_t kUcRowsOfLayout = ~0u;   // Conds::kDenyRows / kAllowRows of a build not generated for one table
 struct GenericConds {
-    static constexpr int kForm = CB_UC_FORM_MASK64;   // the condition word may use all 64 bits
+    // the condition word may use all 64 bits; a complement-coded image gets its (at most 31) bits in the low half and their
+    // complement in the high half, so that the form-1 test reads the need-false mask against the complement
+    static constexpr int kForm = CB_UC_FORM_MASK64;
     static constexpr uint32_t kDenyRows = kUcRowsOfLayout, kAllowRows = kUcRowsOfLayout;   // the image's form is read at run time
     static constexpr uint32_t kListSlots = 0;   // no register-resident lists: no heap prefetch (cb_kernels.h: check_uc_body)
     template <typename Cols>
@@ -4919,20 +4924,21 @@ struct GenericConds {
             slow |= (r & 4u) != 0;
             val |= (uint64_t)(r & 1u) << u;
         }
-        CondWord w; w.lo = val; w.hi = 0;
+        CondWord w; w.lo = t.L->uc_complement ? val | (uint64_t)~(uint32_t)val << 32 : val; w.hi = 0;
         return w;
     }
 };
 
-// (action x role column) pairs of one row if its conditions hold: a needed condition bit that is clear zeroes the role columns
-CB_HD uint32_t cond_bit(const CondWord v, uint32_t u) { return (uint32_t)(((u & 64u) ? v.hi : v.lo) >> (u & 63u)) & 1u; }
-// shift: the row's role field in the role table, below the bits of RP
+// condition bit u of the word, or (neg = 1) its complement
+CB_HD uint32_t cond_bit(const CondWord v, uint32_t u, uint32_t neg) { return ((uint32_t)(((u & 64u) ? v.hi : v.lo) >> (u & 63u)) & 1u) ^ neg; }
+// (action x role column) pairs of one row if its conditions hold: a needed condition bit that is clear, or a condition bit
+// needed clear that is set, zeroes the role columns.  shift: the row's role field in the role table, below the bits of RP
 template <typename RP, int kForm>
 CB_HD uint32_t uc_row_pairs(const U4 r, const RP rp, const CondWord v, const uint32_t role_all, const uint32_t shift) {
     const uint32_t vlo = (uint32_t)v.lo, vhi = (uint32_t)(v.lo >> 32);
-    const uint32_t miss = kForm == CB_UC_FORM_MASK32   ? r.y & ~vlo
+    const uint32_t miss = kForm == CB_UC_FORM_MASK32   ? (r.y & ~vlo) | (r.z & vlo)
                           : kForm == CB_UC_FORM_MASK64 ? (r.y & ~vlo) | (r.z & ~vhi)
-                                                       : (cond_bit(v, r.y & 0xFFu) & cond_bit(v, (r.y >> 8) & 0xFFu)) ^ 1u;
+                                                       : (cond_bit(v, r.y & 0xFFu, 0u) & cond_bit(v, (r.y >> 8) & 0xFFu, 0u)) ^ 1u;
     const uint32_t rc = miss ? 0u : (uint32_t)(rp >> shift) & role_all;
     return r.x * rc;
 }
@@ -5160,9 +5166,9 @@ CB_HD bool eval_request_uc_meta(const TableView t, const BatchView &b, const Col
         for (uint32_t l = 0; l <= top && s != CB_NONE32; l++) {
             const U4 m = ld16(side + bm_base + s);   // {first derived-role record, end, .., ..}
             for (uint32_t e = m.x; e < m.y; e++) {
-                const U4 dr = ld16(side + e);        // {name bit, condition | any role << 31, parent roles lo, hi}
+                const U4 dr = ld16(side + e);        // {name bit, condition bit | needed clear << 30 | any role << 31, parent roles lo, hi}
                 const bool hit = (dr.y >> 31) != 0 || ((((uint64_t)dr.w << 32) | dr.z) & req_roles) != 0;
-                edr |= (uint64_t)(hit && cond_bit(val, dr.y & 0x7FFFFFFFu)) << dr.x;
+                edr |= (uint64_t)(hit && cond_bit(val, dr.y & 0x3FFFFFFFu, (dr.y >> 30) & 1u)) << dr.x;
             }
             s = ld16(chain + s).w;
         }

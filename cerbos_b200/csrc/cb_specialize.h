@@ -435,9 +435,11 @@ inline std::string translate_program(const uint32_t *code_words, uint32_t code_o
 // For tables whose blocks differ in shape the per-shape inlining above explodes; their DISTINCT conditions are few.
 // generate_uc() emits `SpecConds`: load() pulls every attribute slot the conditions read into registers (all loads in
 // flight at once, coalesced), operator() evaluates every distinct DNF term once (shared between conditions) and
-// combines them into the request's condition word.  Rows stay data (16-byte records walked by cb::uc_walk,
+// combines them into the request's condition word, one bit per condition record of the image (a complement-coded image:
+// per base condition, which a condition and its negation share).  Rows stay data (16-byte records walked by cb::uc_walk,
 // unrolled over the image's DENY and ALLOW segment slots).
-// uc: the compact image (cb_uc.h) and its layout.  "" = does not qualify (a distinct condition without flat form ...).
+// uc: the compact image (cb_uc.h) and its layout; n_uconds: its distinct conditions (cbuc::Image::n_uconds).  "" = does
+// not qualify (a distinct condition without flat form ...).
 struct UcLimits {
     uint32_t max_terms = 512;   // distinct terms
 };
@@ -452,10 +454,13 @@ inline UcSource generate_uc(const uint8_t *uc_image, const uint32_t *off, uint32
     if (n_uconds == 0 || n_uconds > 127) return out;
     const uint32_t *const_words = reinterpret_cast<const uint32_t *>(uc_image + off[CB_SEC_CONSTS]);   // cb_const: {tag, pad, bits}
     Atoms atoms;
-    std::vector<std::string> formula(n_uconds + 1);   // per distinct condition without flat form: boolean formula over atoms
-    const uint32_t *uconds = reinterpret_cast<const uint32_t *>(uc_image + uc_conds_off);    // [n_uconds + 1] x {code_off, code_len, flat_off, flat_info}
-    // record 0 (cb_uc.h): {rows the walk visits per scope, DENY slots, ALLOW slots of the segment form (0 / 0: row ranges), 0}
+    const uint32_t *uconds = reinterpret_cast<const uint32_t *>(uc_image + uc_conds_off);    // [n_bits + 1] x {code_off, code_len, flat_off, flat_info}
+    // record 0 (cb_uc.h): {rows the walk visits per scope, DENY slots, ALLOW slots of the segment form (0 / 0: row ranges),
+    // complement-coded: the base conditions (one record and one bit each), else 0: one record per distinct condition}
     const uint32_t scope_rows = uconds[0], deny_rows = uconds[1], allow_rows = uconds[2];
+    const uint32_t n_bits = uconds[3] ? uconds[3] : n_uconds;
+    const uint32_t *base_of = uconds[3] ? uconds + 4 * (n_bits + 1) : nullptr;   // distinct condition - 1 -> base number | negated << 31
+    std::vector<std::string> formula(n_bits + 1);   // per condition without flat form: boolean formula over atoms
     const uint32_t *code = reinterpret_cast<const uint32_t *>(uc_image + off[CB_SEC_CODE]);
     const uint64_t *consts = reinterpret_cast<const uint64_t *>(uc_image + off[CB_SEC_CONSTS_V64]);
     const uint64_t *theap = reinterpret_cast<const uint64_t *>(uc_image + off[CB_SEC_THEAP]);
@@ -467,7 +472,7 @@ inline UcSource generate_uc(const uint8_t *uc_image, const uint32_t *off, uint32
     auto is_slot_kind = [](uint32_t kind) { return kind == CB_OPK_SLOT || kind == CB_OPK_SLOT_ELEM || kind == CB_OPK_SLOT_SIZE; };
     auto use_slot = [&](uint32_t kind, uint32_t v) { if (is_slot_kind(kind) && v < ns) slot_used[v] = true; };
     auto v64_tag = [](uint64_t b) { const uint32_t top = (uint32_t)(b >> 48); return (top & 0xFFF0u) == 0xFFF0u ? (top & 0xFu) : 0u; };
-    for (uint32_t u = 1; u <= n_uconds; u++) {
+    for (uint32_t u = 1; u <= n_bits; u++) {
         const uint32_t *cd = uconds + 4 * u;
         if (cd[3] == 0 || ((cd[3] >> 16) & 0xFF) != CB_FLAT_DNF) {
             formula[u] = translate_program(code, cd[0], cd[1], const_words, n_consts, ns, atoms);
@@ -799,7 +804,12 @@ inline UcSource generate_uc(const uint8_t *uc_image, const uint32_t *off, uint32
         if (reg(v)) s += "        case " + std::to_string(v) + "u: return s" + std::to_string(v) + ";\n";
     s += "        default: return v < " + std::to_string(ns) + "u ? g.slot(v) : (uint64_t)(CB_V64_BOX_BASE | CB_V64_ERROR) << 48;\n        }\n    }\n};\n";
     s += "struct SpecConds {\n    static constexpr uint32_t n_strpred = " + std::to_string(n_pred_bits) + "u;\n";
-    s += std::string("    static constexpr int kForm = ") + (n_uconds <= 31 ? "CB_UC_FORM_MASK32" : n_uconds <= 63 ? "CB_UC_FORM_MASK64" : "CB_UC_FORM_INDEX") + ";   // how the rows name their conditions\n";
+    s += std::string("    static constexpr int kForm = ") + (n_bits <= 31 ? "CB_UC_FORM_MASK32" : n_bits <= 63 ? "CB_UC_FORM_MASK64" : "CB_UC_FORM_INDEX") + ";   // how the rows name their conditions\n";
+    if (base_of) {   // complement-coded image: the rows need each base condition true or false
+        s += "    // " + std::to_string(n_uconds) + " distinct conditions on " + std::to_string(n_bits) + " base conditions, one bit each:\n";
+        for (uint32_t d = 0; d < n_uconds; d++)
+            s += "    // distinct condition " + std::to_string(d + 1) + ": " + (base_of[d] >> 31 ? "!" : "") + "base condition " + std::to_string(base_of[d] & 0x7FFFFFFFu) + "\n";
+    }
     s += "    static constexpr uint32_t kScopeRows = " + std::to_string(scope_rows) + "u;   // rows the walk visits per scope (cb::uc_walk)\n";
     s += "    static constexpr uint32_t kDenyRows = " + std::to_string(deny_rows) + "u, kAllowRows = " + std::to_string(allow_rows) +
          "u;   // segment slots (0 / 0: row ranges)\n";
@@ -897,21 +907,23 @@ inline UcSource generate_uc(const uint8_t *uc_image, const uint32_t *off, uint32
         atom_src += "        slow |= c.unsupported != 0;   // a value the device forms cannot hold: the general kernel reports it\n";
     } else atom_src += "        (void)n;\n";
     std::string typed_src;
-    std::vector<std::string> cond_src(n_uconds + 1);   // per distinct condition: its tri-state block, or its program line
+    std::vector<std::string> cond_src(n_bits + 1);   // per condition bit: its tri-state block, or its program line
+    // the bit of each record; in the 32-bit form the upper half of the word stays zero
+    const std::string what = base_of ? "base condition " : "distinct condition ", cast = n_bits <= 31 ? "(uint32_t)" : "(uint64_t)";
     if (typed) {
         typed_src += "        if (uc_typed(cols.typed)) {   // every term a plain boolean: no error, no deferral\n";
         for (uint32_t q = 0; q < terms.size(); q++) typed_src += "            const bool t" + std::to_string(q) + " = " + tterm[q] + ";\n";
     }
-    for (uint32_t u = 1; u <= n_uconds; u++) {
+    for (uint32_t u = 1; u <= n_bits; u++) {
         const uint32_t *cd = uconds + 4 * u;
         const std::string word = u < 64 ? "val.lo" : "val.hi", sh = std::to_string(u & 63u);
         if (!formula[u].empty()) {
-            cond_src[u] = "        " + word + " |= (uint64_t)(" + formula[u] + ") << " + sh + ";   // distinct condition " + std::to_string(u) + " (program)\n";
+            cond_src[u] = "        " + word + " |= " + cast + "(" + formula[u] + ") << " + sh + ";   // " + what + std::to_string(u) + " (program)\n";
             continue;
         }
         const uint32_t nt = cd[3] & 0xFFFFu, negate = (cd[3] >> 24) & 1u;
         std::string &c = cond_src[u];
-        c += in + "{   // distinct condition " + std::to_string(u) + "\n" + in + "    bool any = false, group = true;\n";
+        c += in + "{   // " + what + std::to_string(u) + "\n" + in + "    bool any = false, group = true;\n";
         std::string any, group;   // typed: an OR of ANDs of literals
         for (uint32_t i = 0; i < nt; i++) {
             const uint32_t *w = code + 2 * (cd[2] + 2 * i);
@@ -925,18 +937,18 @@ inline UcSource generate_uc(const uint8_t *uc_image, const uint32_t *off, uint32
                 group.clear();
             }
         }
-        c += in + "    " + word + std::string(" |= (uint64_t)(any != ") + (negate ? "true" : "false") + ") << " + sh + ";\n" + in + "}\n";
+        c += in + "    " + word + " |= " + cast + "(any != " + (negate ? "true" : "false") + ") << " + sh + ";\n" + in + "}\n";
         if (any.empty()) any = "false";
-        typed_src += "            " + word + " |= (uint64_t)(" + (negate ? "!(" + any + ")" : any) + ") << " + sh + ";   // condition " + std::to_string(u) + "\n";
+        typed_src += "            " + word + " |= " + cast + "(" + (negate ? "!(" + any + ")" : any) + ") << " + sh + ";   // " + (base_of ? what : std::string("condition ")) + std::to_string(u) + "\n";
     }
     if (typed) {
         s += atom_src + "        CondWord val; val.lo = 1ull; val.hi = 0ull;\n" + typed_src + "        } else {   // the tri-state terms on the slot words, reloaded (cols.slot)\n" + tri;
-        for (uint32_t u = 1; u <= n_uconds; u++) if (formula[u].empty()) s += cond_src[u];
+        for (uint32_t u = 1; u <= n_bits; u++) if (formula[u].empty()) s += cond_src[u];
         s += "        }\n";
-        for (uint32_t u = 1; u <= n_uconds; u++) if (!formula[u].empty()) s += cond_src[u];
+        for (uint32_t u = 1; u <= n_bits; u++) if (!formula[u].empty()) s += cond_src[u];
     } else {
         s += tri + atom_src + "        CondWord val; val.lo = 1ull; val.hi = 0ull;\n";
-        for (uint32_t u = 1; u <= n_uconds; u++) s += cond_src[u];
+        for (uint32_t u = 1; u <= n_bits; u++) s += cond_src[u];
     }
     s += "        return val;\n    }\n};\n}  // namespace cb\n";
     out.src = s;

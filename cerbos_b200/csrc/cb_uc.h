@@ -4,7 +4,8 @@
 // keeps one compiled condition per rule (ruletable.go:105-416).  Across a policy set the same conditions recur: shared
 // derived roles, the same ownership / tenancy test on every resource kind.  This builder
 //   * numbers the DISTINCT conditions of the table 1..U (same DNF term list, or -- no flat form -- same bytecode program),
-//   * rewrites every row to {original index, role, effect, mask of the condition bits it needs} (16 bytes, DENY rows first
+//     or, where that fits 31 bits, their BASE conditions (a condition and its negation share one, see build()),
+//   * rewrites every row to {original index, role, effect, masks of the condition bits it needs} (16 bytes, DENY rows first
 //     per block) and, where they fit, lays the rows out in fixed per-block DENY and ALLOW segments of slots,
 //   * copies only the sections the unique-condition kernels read into a compact image (C3: 49 KB blob -> ~10 KB),
 // so that a kernel can evaluate every distinct condition of a request once, with all lanes in lock step, and walk the
@@ -26,6 +27,8 @@ namespace cbuc {
 
 constexpr uint32_t kMaxUconds = 127;      // bit 0 of the condition word is "no condition"
 constexpr uint32_t kMaxMaskUconds = 63;   // up to here rows carry need MASKS; above, the two condition NUMBERS (cb_core.h: CB_UC_FORM_INDEX)
+constexpr uint32_t kMaxComplementBits = 31;   // complement-coded rows: base conditions of one 32-bit condition word
+constexpr uint32_t kNegated = 1u << 31;   // ucond_of_gid: the condition holds where its base condition does not
 
 struct Image {
     bool ok = false;
@@ -33,12 +36,14 @@ struct Image {
     std::vector<uint8_t> bytes;         // compact image (16-byte aligned sections)
     cb::TableLayout lay{};              // offsets into `bytes` + the dims of the source layout
     uint32_t n_uconds = 0, n_flat = 0;  // distinct conditions; how many of them have a flat (DNF) form
+    uint32_t n_bits = 0;                // condition records of the image, one bit of the condition word each (see build())
+    bool complement = false;            // the records are base conditions: rows need each of theirs true or false
     // programs among the conditions, or rows in index form: only the run-time specialised kernel can evaluate the image
-    bool needs_spec() const { return n_flat != n_uconds || n_uconds > kMaxMaskUconds; }
+    bool needs_spec() const { return n_flat != n_uconds || n_bits > kMaxMaskUconds; }
     uint32_t scope_rows = 0;            // rows the walk visits in one scope: deny_rows + allow_rows, else the longest row range
     uint32_t deny_rows = 0, allow_rows = 0;   // slots of every block's DENY / ALLOW segment (0 / 0: row ranges, see build())
     uint32_t n_gids = 0, n_gids_flat = 0;   // table conditions (per-block lists), and how many of them have a flat form
-    std::vector<uint32_t> ucond_of_gid; // table condition id -> distinct condition number (1..U)
+    std::vector<uint32_t> ucond_of_gid; // table condition id -> its condition bit (1..n_bits), | kNegated: it needs the bit clear
 };
 
 // image: the table image (blob bytes); off / len: section offset and byte length by section id; lay: its layout
@@ -54,11 +59,18 @@ inline Image build(const uint8_t *image, const uint32_t *off, const uint64_t *le
         out.why = "section sizes do not match META";
         return out;
     }
-    // distinct conditions
-    std::map<std::tuple<uint32_t, uint32_t, uint32_t>, uint32_t> ids;
-    std::vector<uint32_t> ucond_rec;   // 4 words per distinct condition; entry 0: {scope_rows, deny_rows, allow_rows, 0}
-    ucond_rec.assign(4, 0);
-    out.ucond_of_gid.assign(n_conds, 0);
+    // Distinct conditions: the same DNF term list (flat_off, flat_info), or -- no flat form -- the same bytecode program.
+    // A flat condition and its final negation (flat_info's negate bit: a top-level `none`, as the REQUIRE_PARENTAL_CONSENT
+    // scopes wrap their conditional ALLOWs) share one BASE condition.  The negation is exact, errors included: a term that
+    // fails is neither true nor false as a literal, so the DNF's `any` is false and `none` holds, as in the reference
+    // (ruletable.go:1425-1441: a failed evaluation does not satisfy; none = not any).  When the base conditions fit one
+    // 32-bit word (bit 0: "no condition") and some condition is negated, the image is COMPLEMENT-coded: one record and one
+    // bit per base condition, and a row needs each of its conditions true (first mask) or false (second mask).  Otherwise
+    // one record and one bit per distinct condition, negated or not, as rows of up to 63 bits of masks or in index form.
+    std::map<std::tuple<uint32_t, uint32_t, uint32_t>, uint32_t> ids, base_ids;
+    std::vector<uint32_t> rec_distinct, rec_base;   // 4 words per distinct / base condition: {code_off, code_len, flat_off, flat_info}
+    std::vector<uint32_t> ucond_of, base_of;        // table condition id -> distinct number; distinct number - 1 -> base number | kNegated
+    ucond_of.assign(n_conds, 0);
     for (uint32_t g = 0; g < n_conds; g++) {
         const uint32_t *cd = conds + 4 * g;   // {code_off, code_len, flat_off, flat_info}
         const bool flat = cd[3] != 0 && ((cd[3] >> 16) & 0xFF) == CB_FLAT_DNF;
@@ -68,22 +80,42 @@ inline Image build(const uint8_t *image, const uint32_t *off, const uint64_t *le
             const uint32_t u = (uint32_t)ids.size() + 1;
             if (u > kMaxUconds) { out.why = "more than 127 distinct conditions"; return out; }
             it = ids.emplace(key, u).first;
-            ucond_rec.insert(ucond_rec.end(), {cd[0], cd[1], flat ? cd[2] : 0u, flat ? cd[3] : 0u});
+            rec_distinct.insert(rec_distinct.end(), {cd[0], cd[1], flat ? cd[2] : 0u, flat ? cd[3] : 0u});
             out.n_flat += flat;
+            const uint32_t neg = flat ? cd[3] & 1u << 24 : 0u;
+            const auto bkey = flat ? std::make_tuple(1u, cd[2], cd[3] & ~neg) : key;
+            auto bt = base_ids.find(bkey);
+            if (bt == base_ids.end()) {
+                bt = base_ids.emplace(bkey, (uint32_t)base_ids.size() + 1).first;
+                rec_base.insert(rec_base.end(), {cd[0], cd[1], flat ? cd[2] : 0u, flat ? cd[3] & ~neg : 0u});
+            }
+            base_of.push_back(bt->second | (neg ? kNegated : 0u));
         }
-        out.ucond_of_gid[g] = it->second;
+        ucond_of[g] = it->second;
         out.n_gids++;
         out.n_gids_flat += flat;
     }
     out.n_uconds = (uint32_t)ids.size();
+    out.complement = base_ids.size() < ids.size() && base_ids.size() <= kMaxComplementBits;
+    out.n_bits = out.complement ? (uint32_t)base_ids.size() : out.n_uconds;
+    out.ucond_of_gid.assign(n_conds, 0);
+    for (uint32_t g = 0; g < n_conds; g++) out.ucond_of_gid[g] = out.complement ? base_of[ucond_of[g] - 1] : ucond_of[g];
+    // the condition section: entry 0 {scope_rows, deny_rows, allow_rows, complement-coded: n_bits, else 0}, one record per
+    // bit, then (complement-coded) one word per distinct condition, base number | kNegated, for the generator's listing
+    std::vector<uint32_t> ucond_rec(4, 0);
+    const std::vector<uint32_t> &recs = out.complement ? rec_base : rec_distinct;
+    ucond_rec.insert(ucond_rec.end(), recs.begin(), recs.end());
+    if (out.complement) ucond_rec.insert(ucond_rec.end(), base_of.begin(), base_of.end());
     // Conditions without a flat form stay in the image as programs: only the run-time specialised kernel evaluates them
     // (cb_specialize.h turns their bytecode into straight-line code); the generic unique-condition kernels defer such
     // requests, so the library uses the image of a table with programs only once its specialised kernel is loaded.
     // rows: DENY rows first inside every block (within a scope every matching row is evaluated and DENY beats ALLOW,
-    // ruletable.go:1083-1118, so the order of rows inside a block is free); 16 bytes each, see cb_core.h
+    // ruletable.go:1083-1118, so the order of rows inside a block is free); 16 bytes each, see cb_core.h.  Words 2 / 3:
+    // the 64-bit need mask (bit 0 always set), or complement-coded the need-true mask (bit 0 always set) and the
+    // need-false mask, or in index form the two condition numbers
     std::vector<uint32_t> urows(4 * (size_t)(n_rows ? n_rows : 1), 0);
     std::vector<uint32_t> ublocks(blocks, blocks + 4 * (size_t)n_blocks);   // {row_start, n_rows, DENY rows, 0}
-    const bool index_form = out.n_uconds > kMaxMaskUconds;
+    const bool index_form = out.n_bits > kMaxMaskUconds;
     for (uint32_t b = 0; b < n_blocks; b++) {
         const uint32_t *bl = blocks + 4 * b;   // {row_start, n_rows, cond_base, n_conds}
         if ((uint64_t)bl[0] + bl[1] > n_rows || (uint64_t)bl[2] + bl[3] > n_conds) { out.why = "block out of range"; return out; }
@@ -96,12 +128,14 @@ inline Image build(const uint8_t *image, const uint32_t *off, const uint64_t *le
                 if ((c && c > bl[3]) || (dc && dc > bl[3])) { out.why = "row condition out of range"; return out; }
                 if (role != CB_ROLE_ANY && role >= 64) { out.why = "role id out of range"; return out; }
                 const uint32_t uc = c ? out.ucond_of_gid[bl[2] + c - 1] : 0, udc = dc ? out.ucond_of_gid[bl[2] + dc - 1] : 0;
-                const uint64_t need = index_form ? 0ull : (1ull | 1ull << uc | 1ull << udc);
+                uint64_t need = 1, need_false = 0;   // mask forms
+                for (const uint32_t x : {uc, udc})
+                    if (!index_form) (x & kNegated ? need_false : need) |= 1ull << (x & ~kNegated);
                 uint32_t *u = urows.data() + 4 * (size_t)at++;
                 u[0] = bl[0] + r;
                 u[1] = (role == CB_ROLE_ANY ? 0xFFu : role) | effect << 8;
                 u[2] = index_form ? (uc | udc << 8) : (uint32_t)need;
-                u[3] = index_form ? 0u : (uint32_t)(need >> 32);
+                u[3] = index_form ? 0u : out.complement ? (uint32_t)need_false : (uint32_t)(need >> 32);
                 n_deny += pass == 0;
             }
         }
@@ -198,6 +232,7 @@ inline Image build(const uint8_t *image, const uint32_t *off, const uint64_t *le
     ucond_rec[0] = out.scope_rows;
     ucond_rec[1] = out.deny_rows;
     ucond_rec[2] = out.allow_rows;
+    ucond_rec[3] = out.complement ? out.n_bits : 0u;
     // compact image: the sections the unique-condition kernels (and the interpreter they may call) read
     out.lay = lay;
     for (auto &o : out.lay.off) o = 0;
@@ -216,7 +251,8 @@ inline Image build(const uint8_t *image, const uint32_t *off, const uint64_t *le
     out.lay.uc_rows_off = append(urows.data(), urows.size() * 4);
     out.lay.uc_chain_off = append(chain.data(), chain.size() * 4);
     out.lay.uc_slots_off = segments ? append(slots.data(), slots.size() * 4) : 0;
-    out.lay.n_uconds = out.n_uconds;
+    out.lay.n_uconds = out.n_bits;
+    out.lay.uc_complement = out.complement;
     out.lay.uc_n_rows = segments ? (uint32_t)slots.size() : (uint32_t)(urows.size() / 4);
     out.lay.uc_deny_rows = out.deny_rows;
     out.lay.uc_allow_rows = out.allow_rows;
@@ -232,7 +268,8 @@ inline Image build(const uint8_t *image, const uint32_t *off, const uint64_t *le
 //     {first derived-role record, end, bit 0: a resource policy of this kind exists from s to the end of the chain |
 //      scope levels from s to the end of the chain << 8 (saturating at CB_MAX_CHAIN + 1), 0}
 //   then the derived roles of every block the map names (DR_OFF / DR_ENTRIES / DR_PARENTS, in block order):
-//     {name bit, distinct condition number (cond_bit; 0: none) | any parent role << 31, parent-role mask over the table roles (lo, hi)}
+//     {name bit, condition bit (cond_bit; 0: none) | it must be clear (complement-coded image) << 30 | any parent role << 31,
+//      parent-role mask over the table roles (lo, hi)}
 // Only for the tables the unique-condition kernels take whose metadata needs nothing but the resource chain: no principal
 // or role policies, no parent roles (so a parent role matches a request role by equality, cb::role_in_pr), no condition
 // reading runtime.effectiveDerivedRoles, and no principal-policy existence bits.
@@ -290,7 +327,8 @@ inline MetaSide build_meta(const uint8_t *image, const uint32_t *off, const uint
                     else if (pr < lay.nR) mask |= 1ull << pr;   // (nR <= 64: cbuc::build)
                 }
                 const uint32_t u = en[1] ? uc.ucond_of_gid[en[1] - 1] : 0u;
-                out.words.insert(out.words.end(), {en[0] & 63u, u | (any ? 1u << 31 : 0u), (uint32_t)mask, (uint32_t)(mask >> 32)});
+                out.words.insert(out.words.end(), {en[0] & 63u, (u & ~kNegated) | (u & kNegated ? 1u << 30 : 0u) | (any ? 1u << 31 : 0u),
+                                                   (uint32_t)mask, (uint32_t)(mask >> 32)});
             }
             end[bid] = (uint32_t)(out.words.size() / 4);
         }
